@@ -1,12 +1,13 @@
 #!/usr/bin/env python
-"""bench.py — EasyAnimateV5.1 sampling hot path on B200 (BASELINE.json metric: denoising-steps/sec @49f·720p bf16).
+"""bench.py — EasyAnimateV5.1 sampling hot path on H100 (BASELINE.json metric: denoising-steps/sec @49f·720p bf16).
 
     python bench.py --gpus N --steps K --warmup W            # our arm (torchrun launches one rank per GPU for N>1)
     python bench.py --impl reference --gpus N --steps K ...  # the reference's own CPU path (oracle port), rank 0 only
+    --dump-outputs DIR                                       # also write the last timed step's latents to DIR/latents.npy
 
 A "step" is ONE scheduler step of the denoise loop WITH classifier-free guidance: two MMDiT forwards (batch of 2), the
 CFG combine and the flow-matching Euler update (pipeline_easyanimate.py:1069-1111).  Workload at N=1: BASELINE
-configs[1] read as SURVEY.md §8(d) resolves it — "7B" synthetic MMDiT (d=3072, 48 heads, 28 layers, 6.87 B params),
+configs[1] resolved to — "7B" synthetic MMDiT (d=3072, 48 heads, 28 layers, 6.87 B params),
 49 frames @720x1280 => latent 13x90x160 => 46 800 video + 256 text tokens, synthetic text embeds, random-init weights.
 
 Topology for N > 1 (one process per GPU): N = 2 -> the two CFG branches on one GPU each (one 6 MB all_gather per step);
@@ -43,11 +44,13 @@ PRESETS = {
 }
 S_TEXT, E_TEXT, GUIDANCE = 256, 3584, 6.0
 METRIC = "denoising-steps/sec @49f·720p bf16 (CFG step = 2 MMDiT forwards)"
+# NVIDIA's H100 SXM data sheet (700 W): the denominators of the roofline fractions when no MEASURED_PEAKS.json is present
+H100_BF16_TFLOPS, H100_HBM_GBS, H100_L2_BYTES = 989.0, 3350.0, 50e6
 _CPU_THREADS = None
 
 
 def dit_flops_per_forward(F, h, w, layers, heads, c_in=16, s_t=S_TEXT, e_text=E_TEXT, inpaint=False):
-    """BASELINE.md §2 closed form (MAC = 2 FLOP; softmax/LN/GELU excluded)."""
+    """Closed form of the MMDiT forward FLOPs (MAC = 2 FLOP; softmax/LN/GELU excluded)."""
     d = heads * 64
     s_v = F * (h // 2) * (w // 2)
     s = s_v + s_t
@@ -66,7 +69,7 @@ def _flop_args(p):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -109,7 +112,7 @@ CPU_SAMPLE = dict(F=1, h=64, w=64, layers=1, heads=48)  # 1 024 video + 256 text
 
 
 def cpu_oracle_rate(seconds_budget: float = 15.0, threads: int | None = None, min_reps: int = 2):
-    """Reference CPU path = the oracle restatement (diffusers is not installable offline, DESIGN.md): one
+    """Reference CPU path = the oracle restatement (diffusers is not installable offline): one
     EasyAnimateDiTBlock-deep model (d=3072, 48 heads) on 1 024 video + 256 text tokens, CFG batch 2, bf16, all host
     cores.  Returns (flop/s, description, cores, per-rep seconds list)."""
     import torch
@@ -230,8 +233,8 @@ def build_vae(dev, tiled=False):
 
 def vae_decode_work(vae, F, h, w):
     """Algorithmic work of AutoencoderKLMagvit.decode for a [1,16,F,h,w] latent, walked over the module structure
-    (SURVEY.md §8d: conv FLOPs = sum 2*(T*H*W)_out*C_out*27*C_in, 1x1x1 without the 27; bytes = each conv's input + output
-    once in bf16).  Returns (conv_flops, attn_flops, bytes)."""
+    (conv FLOPs = sum 2*(T*H*W)_out*C_out*27*C_in, 1x1x1 without the 27; bytes = each conv's input + output once in bf16).
+    Returns (conv_flops, attn_flops, bytes)."""
     fl, by, at = 0, 0, 0
     dec = vae.decoder
 
@@ -296,8 +299,8 @@ def vae_lines(preset, dev, peaks, reps=3):
     z = (torch.randn((1, 16, F, h, w), device=dev) / 0.7125).to(bf16)
     conv_fl, attn_fl, nbytes, (T, H, W) = vae_decode_work(vae, F, h, w)
     mpix = T * H * W / 1e6
-    peak_tf = peaks.get("bf16_tflops_sustained", 1400.0)
-    peak_bw = peaks.get("hbm_gbs", 6650.0)
+    peak_tf = peaks.get("bf16_tflops_sustained", H100_BF16_TFLOPS)
+    peak_bw = peaks.get("hbm_gbs", H100_HBM_GBS)
     out = {}
     ms, y = time_cuda(lambda: vae.decode(z).sample, reps)
     out["untiled"] = {"value": mpix / ms * 1e3, "unit": "MPix/s", "ms": ms, "frames": T, "resolution": [H, W],
@@ -306,7 +309,8 @@ def vae_lines(preset, dev, peaks, reps=3):
                                    "frac": (conv_fl + attn_fl) / ms / 1e9 / peak_tf, "conv_tflop": conv_fl / 1e12,
                                    "attn_tflop": attn_fl / 1e12, "algorithmic_gb": nbytes / 1e9,
                                    "hbm_gbs_algorithmic": nbytes / ms / 1e6, "hbm_frac": nbytes / ms / 1e6 / peak_bw,
-                                   "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained / hbm_gbs (of measured)" if peaks else "fallback"}}
+                                   "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained / hbm_gbs (of measured)" if peaks else
+                                                  "H100 SXM data sheet (dense BF16, HBM3 at 700 W)"}}
     del y
     # end to end with host buffers
     z_host = torch.empty(z.shape, dtype=bf16, pin_memory=True).copy_(z * 0.7125)
@@ -333,9 +337,9 @@ def vae_lines(preset, dev, peaks, reps=3):
 
 
 def torch_gpu_baseline(preset, dev, steps=2, warmup=1, with_vae=True):
-    """The in-box baseline SURVEY.md §8(d) asks for: the SAME config and step through stock PyTorch on this GPU - the
+    """The in-box baseline: the SAME config and step through stock PyTorch on this GPU - the
     oracle's modules (nn.Linear -> cuBLAS, F.scaled_dot_product_attention -> flash/cuDNN, LayerNorm/GELU eager kernels),
-    i.e. what the reference executes when handed a B200.  Baseline leg: never the product path."""
+    i.e. what the reference executes when handed this GPU.  Baseline leg: never the product path."""
     import torch
     from oracle import dit
     bf16 = torch.bfloat16
@@ -376,7 +380,7 @@ def torch_gpu_baseline(preset, dev, steps=2, warmup=1, with_vae=True):
         ms = e0.elapsed_time(e1) / steps
         res = {"value": 1e3 / ms, "unit": "steps/s", "ms_per_step": ms, "steps": steps, "warmup": warmup,
                "impl": f"oracle/dit.py modules on cuda, torch {torch.__version__} eager: cuBLAS linears, F.scaled_dot_product_attention, "
-                       "eager LayerNorm/GELU/RoPE (what the reference's modules execute on a B200)",
+                       "eager LayerNorm/GELU/RoPE (what the reference's modules execute on this GPU)",
                "model_tflops": 2 * dit_flops_per_forward(**_flop_args(preset)) / ms / 1e9, "finite": bool(torch.isfinite(lat).all())}
         del m, lat, emb
         torch.cuda.empty_cache()
@@ -415,17 +419,6 @@ def torch_gpu_baseline(preset, dev, steps=2, warmup=1, with_vae=True):
     return res
 
 
-def load_traffic(kernel: str, key: str):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed `ncu --set full` capture
-    (profiles/ncu_traffic.json, written by tools/ncu_summary.py from the .ncu-rep); None when no capture matches."""
-    try:
-        t = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json")))
-        e = t[kernel][key]
-        return e["dram_read_bytes"] + e["dram_write_bytes"], e.get("source")
-    except Exception:
-        return None, None
-
-
 def run_steps(sampler, latents, embeds, rope, n, step_i, inpaint=None):
     for _ in range(n):
         latents = sampler.step(latents, step_i, embeds, rope, inpaint)
@@ -443,9 +436,14 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-vae", action="store_true")
     ap.add_argument("--no-secondary", action="store_true", help="skip the 12B / I2V / torch-baseline secondary lines")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="native arm (--impl ours) only: write the latents the last timed step "
+                    "returned to DIR/latents.npy (float32; weights and inputs are seeded, so runs with the same arguments can be "
+                    "compared output for output)")
     args = ap.parse_args()
     preset = PRESETS[args.preset]
     if args.impl == "reference":
+        if args.dump_outputs:
+            ap.error("--dump-outputs applies to the native arm only: the reference arm times a bounded CPU sample, not the workload")
         return run_reference_arm(args, preset)
 
     import torch
@@ -553,6 +551,10 @@ def main():
     ms_total, launches, attn_ms, latents, step_i = timed_steps(sampler, latents, embeds, rope, inpaint, args.steps, args.warmup, True,
                                                                clocks=clocks)
     clock_info = clocks.stop()
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "latents.npy"), latents.float().cpu().numpy())
 
     # ---- end to end through the public API with HOST buffers (H2D inputs + D2H result every step)
     lat_host = torch.empty(latents.shape, dtype=bf16, pin_memory=True).copy_(latents)
@@ -577,8 +579,8 @@ def main():
 
     line = None
     if rank == 0:
-        peak_tf = peaks.get("bf16_tflops_sustained", 1400.0)
-        peak_src = "MEASURED_PEAKS.json bf16_tflops_sustained" if peaks else "fallback 1.4 PFLOP/s sustained (B200_PROFILING.md)"
+        peak_tf = peaks.get("bf16_tflops_sustained", H100_BF16_TFLOPS)
+        peak_src = "MEASURED_PEAKS.json bf16_tflops_sustained" if peaks else "H100 SXM data sheet, dense BF16 at 700 W"
         S = F * (h // 2) * (w // 2) + S_TEXT
         B_attn = 2 if cfg_group is None else 1
         heads_attn = preset["heads"] // sp  # Ulysses: heads sharded inside attention
@@ -587,7 +589,6 @@ def main():
         achieved = attn_flops / (attn_avg_ms * 1e-3) / 1e12 if attn_avg_ms else None
         flops_step = 2 * dit_flops_per_forward(**_flop_args(preset))
         act_bytes = B_attn * S * preset["heads"] * 64 * 2  # one [B, S, d] bf16 activation
-        traffic, traffic_src = load_traffic("attn6_kernel", f"B{B_attn}_H{heads_attn}_S{S}")
         if world == 1:
             par = "single GPU (CFG batch 2)"
         elif single_video:
@@ -603,7 +604,7 @@ def main():
                        "params": n_params, "latent": [1, 16, F, h, w], "video": f"{4 * (F - 1) + 1}f {h * 8}x{w * 8}",
                        "tokens": S, "text_tokens": S_TEXT, "guidance_scale": GUIDANCE, "scheduler": "flow-match Euler shift=1",
                        "parallelism": par,
-                       "l2": ("inputs_exceed_L2" if act_bytes > 126e6 else "inputs_fit_L2 (not a timing configuration)") +
+                       "l2": ("inputs_exceed_L2" if act_bytes > H100_L2_BYTES else "inputs_fit_L2 (not a timing configuration)") +
                              f" (one activation tensor of a forward is {act_bytes / 1e6:.0f} MB, weights {n_params * 2 / 1e9:.1f} GB)",
                        "tflop_per_step": flops_step / 1e12,
                        "parity_criterion": "tests assert err(ours, fp32 truth) <= 1.5 x err(bf16 oracle, fp32 truth) + 2e-3 per module "
@@ -617,7 +618,6 @@ def main():
             "roofline": {"kernel": "a6::attn6_kernel (joint text+video attention, hd=64, ea_attn_args.variant 0x%x)" % ops.ATTN_VARIANT,
                          "bound": "tensor", "achieved": achieved, "peak": peak_tf, "unit": "TFLOP/s",
                          "frac": (achieved / peak_tf) if achieved else None, "peak_source": peak_src + " (of measured)",
-                         "traffic": traffic, "traffic_source": traffic_src,
                          "traffic_algorithmic": 4.0 * B_attn * heads_attn * S * 64 * 2,
                          "launches_timed": len(attn_ms), "avg_ms": attn_avg_ms, "flops_per_launch": attn_flops,
                          "share_of_step": (sum(attn_ms) / ms_total) if attn_ms else None},
@@ -627,7 +627,7 @@ def main():
     #      decode_latents, float32 frames in host memory (pipeline_easyanimate.py:1052-1149 after the text encoder)
     if rank == 0 and world == 1 and not args.no_vae:
         k_e2e = min(args.steps, 4)
-        vae_e = build_vae(dev)
+        vae_e = build_vae(dev, tiled=True)  # untiled, the decode and the resident 7B model exceed 80 GB
         sampler.vae = vae_e
         Tf = 4 * (F - 1) + 1
         frames = torch.empty((1, 3, Tf, 8 * h, 8 * w), dtype=torch.float32, pin_memory=True)
@@ -651,7 +651,7 @@ def main():
         ms_call = g0.elapsed_time(g1)
         line["e2e_video"] = {"steps": k_e2e, "ms": ms_call, "wall_s": wall, "frames_bytes_to_host": frames.numel() * 4,
                              "steps_per_s_including_decode": k_e2e / ms_call * 1e3, "finite": bool(torch.isfinite(frames).all()),
-                             "what": f"{k_e2e} CFG steps + decode_latents (untiled) + float32 frames [1,3,{Tf},{8 * h},{8 * w}] in pinned "
+                             "what": f"{k_e2e} CFG steps + decode_latents (reference tiling) + float32 frames [1,3,{Tf},{8 * h},{8 * w}] in pinned "
                                      "host memory, inputs from pinned host memory; a 50-step call = 50 x ms_per_step + the decode tail"}
         sampler.vae = None
         del vae_e, frames
@@ -698,9 +698,11 @@ def main():
             # the I2V pipeline's one-off conditioning encode (configs[4]): 49 frames at 1024x1024
             try:
                 x = (torch.rand((1, 3, 49, 1024, 1024), device=dev) * 2 - 1).to(bf16)
+                vae.use_tiling_encoder = True  # the reference's tiled encode: untiled, 49 frames at 1024^2 exceed 80 GB
                 ms_enc, post = time_cuda(lambda: vae.encode(x).latent_dist.mode(), 2)
+                vae.use_tiling_encoder = False
                 secondary["R1024_12B_I2V"]["vae_encode"] = {"ms": ms_enc, "MPix_per_s": 49 * 1024 * 1024 / 1e6 / ms_enc * 1e3,
-                                                            "input": [1, 3, 49, 1024, 1024], "latent": list(post.shape)}
+                                                            "input": [1, 3, 49, 1024, 1024], "latent": list(post.shape), "tiled": True}
                 del x, post
             except Exception as e:
                 secondary["R1024_12B_I2V"]["vae_encode"] = {"unavailable": f"{type(e).__name__}: {str(e)[:160]}"}

@@ -1,4 +1,4 @@
-"""easyanimate_b200 — B200-native (sm_100a) implementation of the EasyAnimateV5.1 sampling hot path.
+"""easyanimate_b200 — H100-native (sm_90a) implementation of the EasyAnimateV5.1 sampling hot path.
 
 Drop-in replacements for the reference's ``easyanimate.models`` name maps (easyanimate/models/__init__.py:6-14):
 importing this package requires the in-tree CUDA library ``libea_b200.so`` (there is no CPU/PyTorch fallback).

@@ -1,15 +1,15 @@
-"""B200-native drop-in for the decode side of ``easyanimate.models.autoencoder_magvit.AutoencoderKLMagvit``.
+"""H100-native drop-in for the decode side of ``easyanimate.models.autoencoder_magvit.AutoencoderKLMagvit``.
 
 Same constructor arguments, ``.config`` surface, ``decode`` signature and decoder ``state_dict`` keys as the reference
 (/root/reference/easyanimate/models/autoencoder_magvit.py:59-505 with the Decoder of
 easyanimate/vae/ldm/models/omnigen_enc_dec.py:339-677).  The nn.Conv3d / nn.GroupNorm / nn.Linear objects only own
 parameters under the reference's key names; decode() runs exclusively on libea_b200.so kernels: channels-last
-activations, tcgen05 implicit-GEMM causal convolutions executed over the WHOLE frame sequence in one launch per
+activations, wgmma implicit-GEMM causal convolutions executed over the WHOLE frame sequence in one launch per
 layer (the reference's per-latent-frame loop with conv caches, omnigen_enc_dec.py:621-629 / common.py:97-141, is
-arithmetically the same convolution), per-frame GroupNorm+SiLU kernels, tcgen05 GEMMs for the 1x1x1 shortcuts and
+arithmetically the same convolution), per-frame GroupNorm+SiLU kernels, wgmma GEMMs for the 1x1x1 shortcuts and
 the mid-block spatial attention.
 
-``encode`` (I2V / inpaint conditioning prep, SURVEY.md section 8(f) rank 2) runs on the same kernels: the encoder's
+``encode`` (I2V / inpaint conditioning prep) runs on the same kernels: the encoder's
 stride-2 convolutions (downsamplers.py:24-96) are the implicit-GEMM kernel with TMA element strides (no wasted FLOPs); the
 stride-1 kernel + strided pick (output (t, i, j) of the strided conv == output (2t, 2i+1, 2j+1) of the stride-1 one) stays
 as an A/B path (EA_ENC_STRIDED=0).  Host logic is checked on CPU against the oracle, which is pinned to the reference's
@@ -393,7 +393,7 @@ class AutoencoderKLMagvit(nn.Module, ConfigMixinLite):
         return dec
 
     def _decode_tiles_parallel(self, z, coords, tl, group):
-        """Tile-parallel decode (SURVEY.md §8e): the reference's tiles are independent decoder passes
+        """Tile-parallel decode: the reference's tiles are independent decoder passes
         (autoencoder_magvit.py:389-402,418-426), so rank r decodes tiles r, r+N, ... of the row-major tile list
         (+ the lower-right corner pass as the last entry) and ONE all-gather of the padded tiles makes every rank
         hold all of them; blending then runs identically on every rank."""

@@ -2,7 +2,7 @@
 
 The reference modules derive from diffusers ``ModelMixin, ConfigMixin`` and decorate ``__init__`` with
 ``@register_to_config`` (easyanimate/models/transformer3d.py:1346-1350, autoencoder_magvit.py:59,93); the pipelines
-then read ``module.config.<name>`` and ``module.config.get(name, default)`` (SURVEY.md §8b).  ``FrozenConfig`` gives
+then read ``module.config.<name>`` and ``module.config.get(name, default)``.  ``FrozenConfig`` gives
 the same read surface without importing diffusers.
 """
 from __future__ import annotations

@@ -1,25 +1,12 @@
-// ea_attn_fwd: argument checks and kernel selection.  The product library carries ONE attention kernel family
-// (attn_tc6.cu).  The earlier generations that lost their A/B measurements (profiles/r01_attn_microbench_*.log) live in
-// tools/attn_ab/ and are linked in only by `EA_ATTN_AB=1 easyanimate_b200/csrc/build.sh` (-DEA_ATTN_AB).
+// ea_attn_fwd: argument checks and kernel selection.  The library carries ONE attention kernel (attn_tc6.cu).
 #include "host.h"
 #include "../../include/ea_b200.h"
 
 namespace ea {
-int launch_attn6(const ea_attn_args* g, int poly, cudaStream_t stream);
-#ifdef EA_ATTN_AB
-int launch_attn1(const ea_attn_args* g, cudaStream_t stream);
-int launch_attn4(const ea_attn_args* g, int poly, cudaStream_t stream);
-int launch_attn9(const ea_attn_args* g, int poly, cudaStream_t stream);
-#endif
+int launch_attn6(const ea_attn_args* g, cudaStream_t stream);
 }  // namespace ea
 
-extern "C" int ea_attn_generations(void) {
-#ifdef EA_ATTN_AB
-  return (1 << 6) | (1 << 1) | (1 << 4) | (1 << 9);
-#else
-  return 1 << 6;
-#endif
-}
+extern "C" int ea_attn_generations(void) { return 1 << 6; }
 
 extern "C" int ea_attn_fwd(const ea_attn_args* g, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
@@ -29,15 +16,7 @@ extern "C" int ea_attn_fwd(const ea_attn_args* g, void* stream_) {
   EA_REQUIRE(g->S_text >= 0 && g->S_text <= g->S, "ea_attn_fwd: bad S_text");
   EA_REQUIRE(g->peers || g->S_text == 0 || g->out_text, "ea_attn_fwd: out_text missing");
   EA_REQUIRE(g->peers || g->S_text == g->S || g->out_video, "ea_attn_fwd: out_video missing");
-  EA_REQUIRE(!g->peers || (g->variant & 0x1100) == 0x100, "ea_attn_fwd: peer outputs exist for the sixth-generation kernel only");
   EA_REQUIRE(g->B * g->H <= 65535, "ea_attn_fwd: B*H exceeds grid.y");
-  if ((g->variant & 0x1100) == 0x100) return ea::launch_attn6(g, (g->variant >> 4) & 7, stream);
-#ifdef EA_ATTN_AB
-  if (g->variant & 0x1000) return ea::launch_attn9(g, (g->variant >> 4) & 7, stream);  // tensor-core row sums, truncated P
-  if ((g->variant & 12) == 12) return ea::launch_attn4(g, (g->variant >> 4) & 7, stream);  // per-block row maximum
-  return ea::launch_attn1(g, stream);
-#else
-  return ea::fail(EA_ERR_INVALID, "ea_attn_fwd: this build carries the sixth-generation kernel only (variant 0x1?c); the A/B "
-                                  "generations need EA_ATTN_AB=1 easyanimate_b200/csrc/build.sh");
-#endif
+  EA_REQUIRE((g->variant & 0x1100) == 0x100, "ea_attn_fwd: this build carries the sixth-generation kernel only (variant 0x1?c)");
+  return ea::launch_attn6(g, stream);
 }

@@ -1,25 +1,12 @@
-// Joint text+video attention forward, sixth generation: the fourth generation's pipeline (two 128-row query tiles per
-// CTA, one TMEM pass over the scores, per-tile MMA issuers, packed fp32x2 softmax, MUFU/FMA exp split) WITHOUT the
-// per-block row maximum on the hot path.
+// Joint text+video attention forward on sm_90a: softmax(Q K^T * scale) V for head_dim 64, one (batch, head) per grid row.
 //
-// ncu's warp-state samples on the fourth generation (profiles/r01_ncu_attn_v4d_hotspots.txt): a softmax warp
-// spends only 54 % of a key block in the exp/pack/store phase; 8 % goes to the four dependent TMEM loads, 12 % to the
-// 65-instruction FMNMX3 chain that must finish before the first exponential can start, 6 % to o_done.  The softmax
-// result does not depend on WHICH reference value is subtracted, only on the same one being used for P and for the
-// row sum, so a block can be exponentiated against the reference kept from earlier blocks (as the lazy-rescale rule
-// already did whenever the maximum grew by < 2^8) and checked afterwards:
-//   * fast pass: chunk c+1 of the scores is loaded from TMEM while chunk c is exponentiated against m_ref; the block's
-//     row sum (every term >= 0, so it bounds every term) and the maximum of the columns that take the polynomial exp2
-//     (whose exponent arithmetic would wrap silently) are checked at the end of the block;
-//   * if any row of the warp fails the check (sum > 2^30, inf or NaN, or a polynomial argument > 64) the warp redoes the
-//     block the classic way from the registers it still holds: true row maximum, rescale O_t and l, exponentiate again.
-//     Block 0 and a ragged last block (masked columns) always take this path.
-// P is written in bf16 (floating point: its relative precision does not depend on the reference), O and l are fp32.
-//
-//   TMEM (512 columns): S_t at 128 t | P_t (packed bf16) at 256 + 64 t | O_t at 384 + 64 t
-//   warps 0-3 / 4-7 : softmax of tile A / B, one query row per thread (setmaxnreg 232; the other warpgroup 40: 256 x 232 + 128 x 40 = 384 x 168)
-//   warp 8          : TMA producer (Q once, K_j / V_j 128-key tiles through 4-stage rings)
-//   warps 9 / 10    : MMA issuer of tile A / B (9 also owns the TMEM allocation);  warp 11: idle
+//   warpgroup 0 (1 thread) : TMA producer — Q once (128 rows), K_j / V_j 128-key tiles through 3-stage rings.
+//   warpgroups 1, 2        : query rows [0,64) / [64,128) of the CTA's tile.  Per key block:
+//                              S = Q K_j^T      wgmma.m64n128k16, both operands in shared memory (SWIZZLE_128B, K-major)
+//                              online softmax   in registers (row max / sum across the 4 threads of a quad), exp2 on MUFU
+//                              O += P V_j       wgmma.m64n64k16, P as bf16 register fragments, V MN-major in shared memory
+// P is rounded to bf16 (as the reference's bf16 attention does), O, the running maximum and the row sums stay fp32.  The
+// two consumer warpgroups run independently, so one's softmax overlaps the other's MMAs.
 #include "common.cuh"
 #include "host.h"
 #include "../../include/ea_b200.h"
@@ -31,15 +18,22 @@ extern void count_launch();
 namespace a6 {
 
 constexpr int kQT = 128;
+constexpr int kKT = 128;
 constexpr int kHD = 64;
-constexpr int kStages = 4;
+constexpr int kStages = 3;
+constexpr int kThreads = 384;
+constexpr int kQBytes = kQT * kHD * 2;
+constexpr int kKVBytes = kKT * kHD * 2;
+constexpr int kOffK = kQBytes;
+constexpr int kOffV = kOffK + kStages * kKVBytes;
+constexpr int kOffBar = kOffV + kStages * kKVBytes;
+constexpr int kTotal = kOffBar + 256 + 1024;
 
 struct Args {
   bf16* out_text;
   bf16* out_video;
   int B, H, S, S_text;
   float scale_log2;
-  uint32_t dep_zero;  // always 0; a value the compiler cannot see through (exp_row_phased)
   // sequence parallelism (ea_attn_peers): this GPU computed heads [head0, head0 + H) of out_heads for ALL tokens; a video
   // token's row goes to the GPU that owns the token (tokens_per_peer each), the text rows to every GPU.  n_peers = 0: local.
   int n_peers, tokens_per_peer, out_heads, head0;
@@ -47,201 +41,68 @@ struct Args {
   bf16* out_text_peers[EA_MAX_PEERS];
 };
 
-// NT query tiles of 128 rows per CTA, key blocks of KT keys.  (2, 128): the layout described above.  (3, 64): three softmax
-// warps per SM sub-partition instead of two (more independent instruction streams to keep the MUFU queue fed across the
-// block-boundary latencies: barrier wait, first TMEM load, verdict, P-store completion), at half the work per block.
-template <int NT, int KT>
-struct Cfg {
-  static constexpr int kThreads = 128 * NT + 128;
-  static constexpr int kQBytes = NT * kQT * kHD * 2;
-  static constexpr int kKBytes = KT * kHD * 2;
-  static constexpr int kVBytes = KT * kHD * 2;
-  static constexpr int kOffQ = 0;
-  static constexpr int kOffK = kOffQ + kQBytes;
-  static constexpr int kOffV = kOffK + kStages * kKBytes;
-  static constexpr int kOffBar = kOffV + kStages * kVBytes;
-  static constexpr int kTotal = kOffBar + 512 + 1024;
-  // TMEM columns: S_t (KT fp32 columns each) | P_t (KT/2 columns of packed bf16 pairs) | O_t (64)
-  static constexpr uint32_t kColP = NT * KT;
-  static constexpr uint32_t kColO = kColP + NT * (KT / 2);
-  static_assert(kColO + NT * kHD <= 512, "TMEM budget");
-  // registers: the producer/MMA warpgroup shrinks to 40, the softmax warpgroups grow to kSoftmaxRegs
-  static constexpr int kSoftmaxRegs = NT == 2 ? 232 : (NT == 3 ? 152 : 96);
-};
-
-EA_DEVICE void tmem_st16(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-EA_DEVICE void tmem_ld32p(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,"
-      "%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
 EA_DEVICE float ex2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-// 2^x for a column pair on the FMA/ALU pipes: x = n + f (round to nearest), degree-3 minimax 2^f, exponent add.
-// Valid for -126 <= x < 128 (clamped below here; the caller guards the upper side).
-EA_DEVICE float2 exp2_poly2(float2 x) {
-  x.x = fmaxf(x.x, -126.0f);
-  x.y = fmaxf(x.y, -126.0f);
-  const float2 y = __fadd2_rn(x, make_float2(12582912.0f, 12582912.0f));
-  const float2 n = __fadd2_rn(y, make_float2(-12582912.0f, -12582912.0f));
-  const float2 f = __ffma2_rn(n, make_float2(-1.0f, -1.0f), x);
-  float2 q = __ffma2_rn(f, make_float2(0.05500892f, 0.05500892f), make_float2(0.24221097f, 0.24221097f));
-  q = __ffma2_rn(q, f, make_float2(0.69328290f, 0.69328290f));
-  q = __ffma2_rn(q, f, make_float2(1.0f, 1.0f));
-  float2 e;
-  e.x = __int_as_float(__float_as_int(q.x) + (__float_as_int(y.x) << 23));
-  e.y = __int_as_float(__float_as_int(q.y) + (__float_as_int(y.y) << 23));
-  return e;
-}
 
-// Hot-loop mbarrier operations on precomputed 32-bit shared addresses.  ncu's source view of the fourth generation
-// showed ~45 instructions per key block re-deriving the barrier addresses (S2R CgaCtaId / SWINHI, align, add) because
-// the compiler rematerialises instead of keeping them; `opaque` hides the derivation so that they stay in registers.
-EA_DEVICE uint32_t opaque(uint32_t x) {
-  asm volatile("" : "+r"(x));
-  return x;
-}
-EA_DEVICE void bar_wait(uint32_t addr, uint32_t parity) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "WAIT_%=:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1, 0x989680;\n\t"
-      "@p bra DONE_%=;\n\t"
-      "bra WAIT_%=;\n\t"
-      "DONE_%=:\n\t}" ::"r"(addr),
-      "r"(parity)
-      : "memory");
-}
-EA_DEVICE void bar_arrive(uint32_t addr) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(addr) : "memory");
-}
-
-// tcgen05.wait::ld that also "touches" the 32 destination registers of the load it completes, so that the compiler
-// cannot schedule their first use above the wait (the load's asm statement already names them as outputs).
-EA_DEVICE void tmem_ld_fence(uint32_t* r) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]), "+r"(r[8]),
-                 "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15]), "+r"(r[16]),
-                 "+r"(r[17]), "+r"(r[18]), "+r"(r[19]), "+r"(r[20]), "+r"(r[21]), "+r"(r[22]), "+r"(r[23]), "+r"(r[24]),
-                 "+r"(r[25]), "+r"(r[26]), "+r"(r[27]), "+r"(r[28]), "+r"(r[29]), "+r"(r[30]), "+r"(r[31])
-               :
-               : "memory");
-}
-
-// fp32 pair -> packed bf16x2.  RN uses F2FP, which issues at 1 per 4 cycles per sub-partition (profiles/
-// r01_issue_mix_microbench.log); TRUNC keeps the high halves with one PRMT (the mean truncation loss of bf16, 2^-8.47,
-// is compensated once, in the epilogue).
-template <bool TRUNC>
-EA_DEVICE uint32_t pack_p(float lo, float hi) {
-  if constexpr (TRUNC) return __byte_perm(__float_as_uint(lo), __float_as_uint(hi), 0x7632);
-  else return pack_bf16x2(lo, hi);
-}
-
-// Column pairs [P0, P1) of one 32-column chunk: e = 2^(s * c - m) with packed fp32x2 arithmetic, POLY of every 4 pairs on
-// the FMA pipe (their raw scores also feed `guard`), the rest on MUFU; row-sum partials in acc2, packed bf16 pairs in pk.
-// PDEN: POLY of every PDEN pairs take the polynomial (4, or 8 / 16 for a finer split between the MUFU and the FMA pipes).
-template <int POLY, int P0, int P1, bool TRUNC = false, int PDEN = 4>
-EA_DEVICE void exp_pairs(const uint32_t* s, float2 c2, float2 nm2, float2* acc2, float& guard, uint32_t* pk) {
-#pragma unroll
-  for (int q = P0; q < P1; ++q) {
-    const float s0 = __uint_as_float(s[2 * q]), s1 = __uint_as_float(s[2 * q + 1]);
-    const float2 x = __ffma2_rn(make_float2(s0, s1), c2, nm2);
-    float2 e;
-    if ((q % PDEN) < POLY) {
-      guard = fmaxf(guard, fmaxf(s0, s1));
-      e = exp2_poly2(x);
+// Stores one 64-wide output row fragment: `v` holds columns 8 jb + c, 8 jb + c + 1 for jb = 0..7 (already normalised).
+EA_DEVICE void store_row(const Args& p, int bh, int srow, int c, const float* v) {
+  if (srow >= p.S) return;
+  const int bb = bh / p.H, h = bh % p.H;
+  bf16* dst;
+  int ndst = 1;  // text rows under sequence parallelism are delivered to every GPU of the group
+  int64_t text_off = 0;
+  if (p.n_peers == 0) {
+    const int64_t d = (int64_t)p.H * kHD;
+    if (srow < p.S_text)
+      dst = p.out_text + ((int64_t)bb * p.S_text + srow) * d + h * kHD;
+    else
+      dst = p.out_video + ((int64_t)bb * (p.S - p.S_text) + (srow - p.S_text)) * d + h * kHD;
+  } else {
+    // Ulysses return exchange fused into the epilogue: [token, head] rows stored straight into the token-major
+    // [B, tokens, out_heads * 64] buffer of the GPU that owns the token (NVLink when it is a peer)
+    const int64_t d = (int64_t)p.out_heads * kHD;
+    if (srow < p.S_text) {
+      text_off = ((int64_t)bb * p.S_text + srow) * d + (int64_t)(p.head0 + h) * kHD;
+      dst = p.out_text_peers[0] + text_off;
+      ndst = p.n_peers;
     } else {
-      e.x = ex2(x.x);
-      e.y = ex2(x.y);
+      const int v = srow - p.S_text;
+      const int owner = v / p.tokens_per_peer;
+      dst = p.out_video_peers[owner] + ((int64_t)bb * p.tokens_per_peer + (v - owner * p.tokens_per_peer)) * d +
+            (int64_t)(p.head0 + h) * kHD;
     }
-    acc2[q & 3] = __fadd2_rn(acc2[q & 3], e);
-    pk[q] = pack_p<TRUNC>(e.x, e.y);
+  }
+#pragma unroll
+  for (int jb = 0; jb < 8; ++jb) {
+    const uint32_t w = pack_bf16x2(v[2 * jb], v[2 * jb + 1]);
+    *reinterpret_cast<uint32_t*>(dst + 8 * jb + c) = w;
+    for (int pr = 1; pr < ndst; ++pr) *reinterpret_cast<uint32_t*>(p.out_text_peers[pr] + text_off + 8 * jb + c) = w;
   }
 }
 
-// The same over a whole 128-column row, but in two PHASES: first every polynomial pair, then every MUFU pair.  A warp
-// stalled at the MUFU queue cannot issue the FMA work queued behind it (in order), so mixing the two kinds pair by pair
-// leaves both pipes half idle; with phases, one tile's FMA-only phase runs under the other tile's MUFU phase (the two
-// softmax warps of a sub-partition belong to different tiles).  `dep_zero` is a runtime zero that chains the MUFU
-// phase's inputs to the last polynomial result so that ptxas cannot merge the phases back together.
-template <int POLY>
-EA_DEVICE void exp_row_phased(const uint32_t* s, float2 c2, float2 nm2, float2* acc2, float& guard, uint32_t* pk,
-                              uint32_t dep_zero) {
-  uint32_t last = 0;
-#pragma unroll
-  for (int q = 0; q < 64; ++q) {
-    if ((q & 3) < POLY) {
-      const float s0 = __uint_as_float(s[2 * q]), s1 = __uint_as_float(s[2 * q + 1]);
-      guard = fmaxf(guard, fmaxf(s0, s1));
-      const float2 e = exp2_poly2(__ffma2_rn(make_float2(s0, s1), c2, nm2));
-      acc2[q & 3] = __fadd2_rn(acc2[q & 3], e);
-      pk[q] = pack_bf16x2(e.x, e.y);
-      last = pk[q];
-    }
-  }
-  const float2 nm2b = make_float2(__uint_as_float(__float_as_uint(nm2.x) | (last & dep_zero)), nm2.y);
-#pragma unroll
-  for (int q = 0; q < 64; ++q) {
-    if ((q & 3) >= POLY) {
-      const float2 x = __ffma2_rn(make_float2(__uint_as_float(s[2 * q]), __uint_as_float(s[2 * q + 1])), c2, nm2b);
-      float2 e;
-      e.x = ex2(x.x);
-      e.y = ex2(x.y);
-      acc2[q & 3] = __fadd2_rn(acc2[q & 3], e);
-      pk[q] = pack_bf16x2(e.x, e.y);
-    }
-  }
-}
-
-template <int POLY, bool PHASED, bool TRUNC, int NT, int KT, int PDEN>
-__global__ void __launch_bounds__(Cfg<NT, KT>::kThreads, 1)
+__global__ void __launch_bounds__(kThreads, 1)
 attn6_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
              const __grid_constant__ CUtensorMap tmap_v, const Args p) {
-  using C = Cfg<NT, KT>;
-  static_assert(!PHASED || (NT == 2 && KT == 128), "the two-phase variant exists for the 2 x 128 layout only");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sQ = smem + C::kOffQ;
-  uint8_t* sK = smem + C::kOffK;
-  uint8_t* sV = smem + C::kOffV;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::kOffBar);
+  uint8_t* sQ = smem;
+  uint8_t* sK = smem + kOffK;
+  uint8_t* sV = smem + kOffV;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kOffBar);
   uint64_t* q_full = bars;
   uint64_t* k_full = bars + 1;
   uint64_t* k_empty = k_full + kStages;
   uint64_t* v_full = k_empty + kStages;
   uint64_t* v_empty = v_full + kStages;
-  uint64_t* s_full = v_empty + kStages;   // [tile]
-  uint64_t* s_free = s_full + NT;         // [tile]
-  uint64_t* p_ready = s_free + NT;        // [tile]
-  uint64_t* o_done = p_ready + NT;        // [tile]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_done + NT);
 
-  const int warp = threadIdx.x >> 5;
+  const int wg = threadIdx.x >> 7;
   const int lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * (NT * kQT);
+  const int q0 = blockIdx.x * kQT;
   const int bh = blockIdx.y;
-  const int nblk = (p.S + KT - 1) / KT;
-  constexpr int kProducerWarp = 4 * NT;      // then one MMA issuer warp per tile
-  constexpr int kFirstIssuer = 4 * NT + 1;
-
-  constexpr uint32_t kColP = C::kColP, kColO = C::kColO;
-  constexpr uint32_t kTmemCols = 512;
+  const int nblk = (p.S + kKT - 1) / kKT;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_q);
@@ -250,328 +111,141 @@ attn6_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__
     mbar_init(q_full, 1);
     for (int i = 0; i < kStages; ++i) {
       mbar_init(&k_full[i], 1);
-      mbar_init(&k_empty[i], NT);  // one tcgen05.commit per tile issuer
+      mbar_init(&k_empty[i], 8);  // lane 0 of each consumer warp
       mbar_init(&v_full[i], 1);
-      mbar_init(&v_empty[i], NT);
-    }
-    for (int i = 0; i < NT; ++i) {
-      mbar_init(&s_full[i], 1);
-      mbar_init(&s_free[i], 128);
-      mbar_init(&p_ready[i], 128);
-      mbar_init(&o_done[i], 1);
+      mbar_init(&v_empty[i], 8);
     }
     fence_mbar_init();
   }
-  if (warp == kFirstIssuer) tmem_alloc(tmem_slot, kTmemCols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp >= kProducerWarp) {
-  // ---- producer / MMA warpgroup: give registers back
-  asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
-  if (warp == kProducerWarp) {
-    if (lane == 0) {
+  if (wg == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (threadIdx.x == 0) {
       // ===== TMA producer =====
-      mbar_arrive_expect_tx(q_full, C::kQBytes);
-#pragma unroll
-      for (int t = 0; t < NT; ++t) tma_load_3d(sQ + t * (kQT * kHD * 2), &tmap_q, q_full, 0, q0 + t * kQT, bh);
+      mbar_arrive_expect_tx(q_full, kQBytes);
+      tma_load_3d(sQ, &tmap_q, q_full, 0, q0, bh);
       int st = 0;
       uint32_t ph = 0;
       for (int j = 0; j < nblk; ++j) {
         mbar_wait(&k_empty[st], ph ^ 1);
-        mbar_arrive_expect_tx(&k_full[st], C::kKBytes);
-        tma_load_3d(sK + st * C::kKBytes, &tmap_k, &k_full[st], 0, j * KT, bh);
+        mbar_arrive_expect_tx(&k_full[st], kKVBytes);
+        tma_load_3d(sK + st * kKVBytes, &tmap_k, &k_full[st], 0, j * kKT, bh);
         mbar_wait(&v_empty[st], ph ^ 1);
-        mbar_arrive_expect_tx(&v_full[st], C::kVBytes);
-        tma_load_3d(sV + st * C::kVBytes, &tmap_v, &v_full[st], 0, j * KT, bh);
+        mbar_arrive_expect_tx(&v_full[st], kKVBytes);
+        tma_load_3d(sV + st * kKVBytes, &tmap_v, &v_full[st], 0, j * kKT, bh);
         if (++st == kStages) { st = 0; ph ^= 1; }
       }
     }
-  } else if (warp < kFirstIssuer + NT) {
-    if (lane == 0) {
-      // ===== MMA issuers: one warp per query tile, independently =====
-      // (one issuer walking the tiles in a fixed order head-of-line blocks: it sits in wait(p_ready[A]) while
-      //  s_free[B] has long fired, the tiles lock IN phase and the TMEM-read and exp phases never overlap.)
-      const int t = warp - kFirstIssuer;
-      constexpr uint32_t idesc_qk = umma_idesc_bf16(kQT, KT, 0, 0);
-      constexpr uint32_t idesc_pv = umma_idesc_bf16(kQT, kHD, 0, 1);  // V: MN-major B operand
-      mbar_wait(q_full, 0);
-      tc_fence_after();
-      auto issue_qk = [&](int t, int j) {
-        const int st = j % kStages;
-        const uint64_t qdesc = umma_desc_sw128(smem_u32(sQ + t * (kQT * kHD * 2)));
-        const uint64_t kdesc = umma_desc_sw128(smem_u32(sK + st * C::kKBytes));
-        const uint32_t d = tmem_base + t * KT;
-#pragma unroll
-        for (int k = 0; k < kHD / 16; ++k) umma_ss(d, qdesc + 2 * k, kdesc + 2 * k, idesc_qk, k != 0);
-        umma_commit(&s_full[t]);
-      };
-      auto issue_pv = [&](int t, int j) {
-        const int st = j % kStages;
-        const uint32_t vaddr = smem_u32(sV + st * C::kVBytes);
-        const uint32_t d = tmem_base + kColO + t * kHD;
-        const uint32_t pa = tmem_base + kColP + t * (KT / 2);
-#pragma unroll
-        for (int k = 0; k < KT / 16; ++k)
-          umma_ts(d, pa + k * 8, umma_desc_sw128_mn(vaddr + k * 2048, C::kVBytes, 1024), idesc_pv, (j | k) != 0);
-        umma_commit(&o_done[t]);
-      };
-      mbar_wait(&k_full[0], 0);
-      tc_fence_after();
-      issue_qk(t, 0);
-      umma_commit(&k_empty[0]);  // K/V stages are released when ALL issuers have committed (barrier count NT)
-      for (int j = 0; j < nblk; ++j) {
-        const int st = j % kStages;
-        const uint32_t par = j & 1;
-        if (j + 1 < nblk) {
-          mbar_wait(&s_free[t], par);  // this tile's softmax has pulled S(j) into registers
-          mbar_wait(&k_full[(j + 1) % kStages], ((j + 1) / kStages) & 1);
-          tc_fence_after();
-          issue_qk(t, j + 1);
-          umma_commit(&k_empty[(j + 1) % kStages]);
-        }
-        mbar_wait(&p_ready[t], par);
-        mbar_wait(&v_full[st], (j / kStages) & 1);
-        tc_fence_after();
-        issue_pv(t, j);
-        umma_commit(&v_empty[st]);
-      }
-    }
-  }
-  } else {
-    // ---- softmax warpgroups: take them
-    if constexpr (NT == 2) asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
-    else if constexpr (NT == 3) asm volatile("setmaxnreg.inc.sync.aligned.u32 152;");
-    // (NT == 4: the kernel is compiled for 96 registers - 65 536 / 640 threads - and the 128 x 56 the other warpgroup releases
-    //  would not cover an increase of all 512 softmax threads past 104: setmaxnreg.inc only draws from the CTA's own pool)
-    // ===== softmax / correction / epilogue: tile t, one query row per thread =====
-    const int t = warp >> 2;
-    const int ew = warp & 3;
-    const int r = ew * 32 + lane;
-    const uint32_t lane_off = uint32_t(ew * 32) << 16;
-    const uint32_t tS = tmem_base + lane_off + t * KT;
-    const uint32_t tP = tmem_base + lane_off + kColP + t * (KT / 2);
-    const uint32_t tO = tmem_base + lane_off + kColO + t * kHD;
-    const uint32_t bar_t = opaque(smem_u32(&s_full[t]));  // s_full[t]; s_free[t], p_ready[t], o_done[t] follow at 8*NT strides
-    constexpr uint32_t kSFree = 8 * NT, kPReady = 16 * NT, kODone = 24 * NT;
-    float m_ref = 0.f;
-    float l = 0.f;
-    const float2 c2 = make_float2(p.scale_log2, p.scale_log2);
-    for (int j = 0; j < nblk; ++j) {
-      bar_wait(bar_t, j & 1);
-      // start the tiles a fraction of a period apart: tile t's first block begins when tile t-1 has pulled its scores
-      if (t > 0 && j == 0) mbar_wait(&s_free[t - 1], 0);
-      tc_fence_after();
-      uint32_t s[KT];
-      uint32_t pk[16], pk2[16];
-      const int valid = p.S - j * KT;  // < KT only in the last block (TMA zero-filled the missing keys)
-      float2 acc2[4] = {{0.f, 0.f}, {0.f, 0.f}, {0.f, 0.f}, {0.f, 0.f}};
-      float guard = -INFINITY;
-      bool redo = (j == 0) || (valid < KT);
-      if (!redo) {
-        // ---- fast pass: exponentiate against the reference kept from earlier blocks.  The P stores trail the
-        // exponentials by one chunk so that the wait for PV_{j-1} (which reads P_t) sits in the middle of the block.
-        const float2 nm2 = make_float2(-m_ref, -m_ref);
-        if constexpr (PHASED) {
-          uint32_t pkr[64];
-          tmem_ld32p(tS, s);
-          tmem_ld32p(tS + 32, s + 32);
-          tmem_ld32p(tS + 64, s + 64);
-          tmem_ld32p(tS + 96, s + 96);
-          tmem_ld_fence(s);
-          tmem_ld_fence(s + 32);
-          tmem_ld_fence(s + 64);
-          tmem_ld_fence(s + 96);
-          tc_fence_before();
-          bar_arrive(bar_t + kSFree);  // S_t may be overwritten by QK_{j+1}
-          exp_row_phased<POLY>(s, c2, nm2, acc2, guard, pkr, p.dep_zero);
-          bar_wait(bar_t + kODone, (j - 1) & 1);  // PV_{j-1} has read P_t
-          tc_fence_after();
-          tmem_st16(tP, pkr);
-          tmem_st16(tP + 16, pkr + 16);
-          tmem_st16(tP + 32, pkr + 32);
-          tmem_st16(tP + 48, pkr + 48);
-        } else if constexpr (KT == 128) {
-          tmem_ld32p(tS, s);
-          tmem_ld_fence(s);
-          tmem_ld32p(tS + 32, s + 32);
-          exp_pairs<POLY, 0, 16, TRUNC, PDEN>(s, c2, nm2, acc2, guard, pk);
-          tmem_ld_fence(s + 32);
-          tmem_ld32p(tS + 64, s + 64);
-          exp_pairs<POLY, 0, 8, TRUNC, PDEN>(s + 32, c2, nm2, acc2, guard, pk2);
-          tmem_ld_fence(s + 64);
-          tmem_ld32p(tS + 96, s + 96);
-          exp_pairs<POLY, 8, 16, TRUNC, PDEN>(s + 32, c2, nm2, acc2, guard, pk2);
-          tmem_ld_fence(s + 96);
-          tc_fence_before();
-          bar_arrive(bar_t + kSFree);  // S_t may be overwritten by QK_{j+1}
-          bar_wait(bar_t + kODone, (j - 1) & 1);  // PV_{j-1} has read P_t
-          tc_fence_after();
-          tmem_st16(tP, pk);
-          tmem_st16(tP + 16, pk2);
-          exp_pairs<POLY, 0, 16, TRUNC, PDEN>(s + 64, c2, nm2, acc2, guard, pk);
-          tmem_st16(tP + 32, pk);
-          exp_pairs<POLY, 0, 16, TRUNC, PDEN>(s + 96, c2, nm2, acc2, guard, pk2);
-          tmem_st16(tP + 48, pk2);
-        } else if constexpr (KT == 32) {
-          // one 32-column chunk per block: four softmax warps per SM sub-partition, a quarter of the work per block
-          tmem_ld32p(tS, s);
-          tmem_ld_fence(s);
-          tc_fence_before();
-          bar_arrive(bar_t + kSFree);  // S_t may be overwritten by QK_{j+1}
-          exp_pairs<POLY, 0, 8, TRUNC, PDEN>(s, c2, nm2, acc2, guard, pk);
-          bar_wait(bar_t + kODone, (j - 1) & 1);  // PV_{j-1} has read P_t
-          tc_fence_after();
-          exp_pairs<POLY, 8, 16, TRUNC, PDEN>(s, c2, nm2, acc2, guard, pk);
-          tmem_st16(tP, pk);
-        } else {
-          static_assert(KT == 64 || KT == 128, "key block of 32, 64 or 128");
-          tmem_ld32p(tS, s);
-          tmem_ld_fence(s);
-          tmem_ld32p(tS + 32, s + 32);
-          exp_pairs<POLY, 0, 16, TRUNC, PDEN>(s, c2, nm2, acc2, guard, pk);
-          tmem_ld_fence(s + 32);
-          tc_fence_before();
-          bar_arrive(bar_t + kSFree);  // S_t may be overwritten by QK_{j+1}
-          exp_pairs<POLY, 0, 8, TRUNC, PDEN>(s + 32, c2, nm2, acc2, guard, pk2);
-          bar_wait(bar_t + kODone, (j - 1) & 1);  // PV_{j-1} has read P_t
-          tc_fence_after();
-          tmem_st16(tP, pk);
-          exp_pairs<POLY, 8, 16, TRUNC, PDEN>(s + 32, c2, nm2, acc2, guard, pk2);
-          tmem_st16(tP + 16, pk2);
-        }
-        const float l_blk = ((acc2[0].x + acc2[0].y) + (acc2[1].x + acc2[1].y)) + ((acc2[2].x + acc2[2].y) + (acc2[3].x + acc2[3].y));
-        const bool ok = (l_blk <= 1073741824.0f) && (POLY == 0 || fmaf(guard, p.scale_log2, -m_ref) <= 64.0f);
-        redo = __any_sync(0xffffffffu, !ok);
-        if (!redo) l += l_blk;
-      } else {
-#pragma unroll
-        for (int c = 0; c < KT / 32; ++c) tmem_ld32p(tS + c * 32, s + c * 32);
-        tmem_ld_wait();
-        tc_fence_before();
-        bar_arrive(bar_t + kSFree);
-        if (valid < KT) {
-#pragma unroll
-          for (int i = 0; i < KT; ++i)
-            if (i >= valid) s[i] = 0xff800000u;  // -inf
-        }
-      }
-      if (redo) {
-        // ---- classic pass from the registers: true row maximum, rescale, exponentiate (block 0, ragged last block, or a
-        // row whose scores outgrew the reference by more than 2^30)
-        float m4[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-#pragma unroll
-        for (int i = 0; i < KT; ++i) m4[i & 3] = fmaxf(m4[i & 3], __uint_as_float(s[i]));
-        const float mx = fmaxf(fmaxf(m4[0], m4[1]), fmaxf(m4[2], m4[3])) * p.scale_log2;
-        if (j == 0) {
-          m_ref = mx;
-        } else {
-          bar_wait(bar_t + kODone, (j - 1) & 1);
-          tc_fence_after();
-          const float m_new = fmaxf(m_ref, mx);
-          const float f = ex2(m_ref - m_new);
-#pragma unroll
-          for (int c = 0; c < 2; ++c) {
-            uint32_t v[32];
-            tmem_ld32(tO + c * 32, v);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] = __float_as_uint(__uint_as_float(v[i]) * f);
-            tmem_st32(tO + c * 32, v);
-          }
-          tmem_st_wait();
-          l *= f;
-          m_ref = m_new;
-        }
-        const float2 nm2 = make_float2(-m_ref, -m_ref);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) acc2[i] = make_float2(0.f, 0.f);
-#pragma unroll 1
-        for (int c = 0; c < KT / 32; ++c) {
-          // (rare path: keep it small - rotate the score registers instead of unrolling the chunks)
-          exp_pairs<POLY, 0, 16, TRUNC, PDEN>(s, c2, nm2, acc2, guard, pk);
-          tmem_st16(tP + c * 16, pk);
-#pragma unroll
-          for (int i = 0; i < KT - 32; ++i) s[i] = s[i + 32];
-        }
-        l += ((acc2[0].x + acc2[0].y) + (acc2[1].x + acc2[1].y)) + ((acc2[2].x + acc2[2].y) + (acc2[3].x + acc2[3].y));
-      }
-      tmem_st_wait();
-      tc_fence_before();
-      bar_arrive(bar_t + kPReady);
-    }
-    bar_wait(bar_t + kODone, (nblk - 1) & 1);
-    tc_fence_after();
-    const float inv_l = (TRUNC ? 1.00282f : 1.0f) / l;
-    const int srow = q0 + t * kQT + r;
-    bf16* dst = nullptr;
-    int ndst = 1;            // text rows under sequence parallelism are delivered to every GPU of the group
-    int64_t text_off = 0;
-    if (srow < p.S) {
-      const int bb = bh / p.H, h = bh % p.H;
-      if (p.n_peers == 0) {
-        const int64_t d = (int64_t)p.H * kHD;
-        if (srow < p.S_text)
-          dst = p.out_text + ((int64_t)bb * p.S_text + srow) * d + h * kHD;
-        else
-          dst = p.out_video + ((int64_t)bb * (p.S - p.S_text) + (srow - p.S_text)) * d + h * kHD;
-      } else {
-        // Ulysses return exchange fused into the epilogue: [token, head] rows of 128 bytes stored straight into the
-        // token-major [B, tokens, out_heads * 64] buffer of the GPU that owns the token (NVLink when it is a peer)
-        const int64_t d = (int64_t)p.out_heads * kHD;
-        if (srow < p.S_text) {
-          text_off = ((int64_t)bb * p.S_text + srow) * d + (int64_t)(p.head0 + h) * kHD;
-          dst = p.out_text_peers[0] + text_off;
-          ndst = p.n_peers;
-        } else {
-          const int v = srow - p.S_text;
-          const int owner = v / p.tokens_per_peer;
-          dst = p.out_video_peers[owner] + ((int64_t)bb * p.tokens_per_peer + (v - owner * p.tokens_per_peer)) * d +
-                (int64_t)(p.head0 + h) * kHD;
-        }
-      }
-    }
-#pragma unroll
-    for (int c = 0; c < 2; ++c) {
-      uint32_t v[32];
-      __syncwarp();
-      tmem_ld32(tO + c * 32, v);
-      tmem_ld_wait();
-      if (dst != nullptr) {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          uint4 w;
-          w.x = pack_bf16x2(__uint_as_float(v[i * 8 + 0]) * inv_l, __uint_as_float(v[i * 8 + 1]) * inv_l);
-          w.y = pack_bf16x2(__uint_as_float(v[i * 8 + 2]) * inv_l, __uint_as_float(v[i * 8 + 3]) * inv_l);
-          w.z = pack_bf16x2(__uint_as_float(v[i * 8 + 4]) * inv_l, __uint_as_float(v[i * 8 + 5]) * inv_l);
-          w.w = pack_bf16x2(__uint_as_float(v[i * 8 + 6]) * inv_l, __uint_as_float(v[i * 8 + 7]) * inv_l);
-          *reinterpret_cast<uint4*>(dst + c * 32 + i * 8) = w;
-          for (int pr = 1; pr < ndst; ++pr) *reinterpret_cast<uint4*>(p.out_text_peers[pr] + text_off + c * 32 + i * 8) = w;
-        }
-      }
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kFirstIssuer) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  // ===== consumers: 64 query rows each; this thread holds rows r and r + 8 of them, columns 8 jb + c, + 1 =====
+  const int cw = wg - 1;
+  const int r = 16 * ((threadIdx.x & 127) >> 5) + (lane >> 2);
+  const int c = 2 * (lane & 3);
+  const float sl2 = p.scale_log2;
+  float o[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  float m[2] = {-INFINITY, -INFINITY};  // running maximum of the scaled scores (log2 domain)
+  float l[2] = {0.f, 0.f};              // this thread's share of the row sums
+
+  mbar_wait(q_full, 0);
+  const uint64_t qdesc = gmma_desc_sw128(smem_u32(sQ + cw * 64 * 128));
+  int st = 0;
+  uint32_t ph = 0;
+  for (int j = 0; j < nblk; ++j) {
+    float s[64];
+    mbar_wait(&k_full[st], ph);
+    const uint64_t kdesc = gmma_desc_sw128(smem_u32(sK + st * kKVBytes));
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < kHD / 16; ++k) wgmma_ss<128>(s, qdesc + 2 * k, kdesc + 2 * k, k != 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence<64>(s);
+    if (lane == 0) mbar_arrive(&k_empty[st]);
+
+    const int valid = p.S - j * kKT;  // < kKT only in the last block (TMA zero-filled the missing keys)
+    if (valid < kKT) {
+#pragma unroll
+      for (int jb = 0; jb < 16; ++jb)
+#pragma unroll
+        for (int e = 0; e < 4; ++e)
+          if (8 * jb + c + (e & 1) >= valid) s[4 * jb + e] = -INFINITY;
+    }
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int jb = 0; jb < 16; ++jb) {
+      mx[0] = fmaxf(mx[0], fmaxf(s[4 * jb], s[4 * jb + 1]));
+      mx[1] = fmaxf(mx[1], fmaxf(s[4 * jb + 2], s[4 * jb + 3]));
+    }
+    float nm[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+      const float m_new = fmaxf(m[h], mx[h] * sl2);
+      const float f = ex2(m[h] - m_new);  // 0 for the first block (m = -inf)
+      l[h] *= f;
+#pragma unroll
+      for (int jb = 0; jb < 8; ++jb) {
+        o[4 * jb + 2 * h] *= f;
+        o[4 * jb + 2 * h + 1] *= f;
+      }
+      m[h] = m_new;
+      nm[h] = -m_new;
+    }
+    // P = 2^(s * scale_log2 - m) as bf16 A fragments of m64n64k16: k-step kk takes key columns [16 kk, 16 kk + 16)
+    uint32_t pa[8][4];
+#pragma unroll
+    for (int jb = 0; jb < 16; ++jb) {
+      const float e0 = ex2(fmaf(s[4 * jb], sl2, nm[0])), e1 = ex2(fmaf(s[4 * jb + 1], sl2, nm[0]));
+      const float e2 = ex2(fmaf(s[4 * jb + 2], sl2, nm[1])), e3 = ex2(fmaf(s[4 * jb + 3], sl2, nm[1]));
+      l[0] += e0 + e1;
+      l[1] += e2 + e3;
+      pa[jb >> 1][2 * (jb & 1)] = pack_bf16x2(e0, e1);
+      pa[jb >> 1][2 * (jb & 1) + 1] = pack_bf16x2(e2, e3);
+    }
+
+    mbar_wait(&v_full[st], ph);
+    const uint32_t vaddr = smem_u32(sV + st * kKVBytes);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < kKT / 16; ++kk) wgmma_rs_tb<64>(o, pa[kk], gmma_desc_sw128(vaddr + kk * 2048, 1024, kKVBytes));
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence<32>(o);
+    if (lane == 0) mbar_arrive(&v_empty[st]);
+    if (++st == kStages) { st = 0; ph ^= 1; }
+  }
+
+  // ===== epilogue: O / l, bf16 rows to the text / video outputs (or the peers') =====
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float lt = l[h];
+    lt += __shfl_xor_sync(0xffffffffu, lt, 1);
+    lt += __shfl_xor_sync(0xffffffffu, lt, 2);
+    const float inv_l = 1.0f / lt;
+    float v[16];
+#pragma unroll
+    for (int jb = 0; jb < 8; ++jb) {
+      v[2 * jb] = o[4 * jb + 2 * h] * inv_l;
+      v[2 * jb + 1] = o[4 * jb + 2 * h + 1] * inv_l;
+    }
+    store_row(p, bh, q0 + cw * 64 + r + 8 * h, c, v);
   }
 }
 
-template <int POLY, bool PHASED, bool TRUNC, int NT = 2, int KT = 128, int PDEN = 4>
 static int launch(const ea_attn_args* g, cudaStream_t stream) {
-  using C = Cfg<NT, KT>;
   const int64_t BH = g->B * g->H;
   CUtensorMap tq, tk, tv;
   uint64_t dims[3] = {(uint64_t)kHD, (uint64_t)g->S, (uint64_t)BH};
   uint64_t strides[2] = {(uint64_t)kHD * 2, (uint64_t)g->S * kHD * 2};
   uint32_t box_q[3] = {kHD, kQT, 1};
-  uint32_t box_kv[3] = {kHD, KT, 1};
+  uint32_t box_kv[3] = {kHD, kKT, 1};
   int rc = make_tmap_bf16(&tq, g->q, 3, dims, strides, box_q, true);
   if (rc) return rc;
   rc = make_tmap_bf16(&tk, g->k, 3, dims, strides, box_kv, true);
@@ -583,7 +257,6 @@ static int launch(const ea_attn_args* g, cudaStream_t stream) {
   p.out_video = reinterpret_cast<bf16*>(g->out_video);
   p.B = (int)g->B; p.H = (int)g->H; p.S = (int)g->S; p.S_text = (int)g->S_text;
   p.scale_log2 = g->scale * 1.4426950408889634f;
-  p.dep_zero = 0;
   if (g->peers != nullptr) {
     const ea_attn_peers* pe = g->peers;
     if (pe->n_peers < 1 || pe->n_peers > EA_MAX_PEERS || pe->tokens_per_peer <= 0 || pe->out_heads < pe->head0 + g->H ||
@@ -596,45 +269,26 @@ static int launch(const ea_attn_args* g, cudaStream_t stream) {
       p.out_text_peers[i] = reinterpret_cast<bf16*>(pe->out_text[i]);
     }
   }
-  auto kern = attn6_kernel<POLY, PHASED, TRUNC, NT, KT, PDEN>;
+  auto kern = attn6_kernel;
   static ::ea::PerDeviceFlag attr_flag;
   const int attr_dev = ::ea::current_device();
   if (!attr_flag.get(attr_dev)) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kTotal);
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kTotal);
     if (e != cudaSuccess) return fail(EA_ERR_CUDA, std::string("cudaFuncSetAttribute(attn6): ") + cudaGetErrorString(e));
     attr_flag.set(attr_dev);
   }
-  dim3 grid((unsigned)((g->S + NT * kQT - 1) / (NT * kQT)), (unsigned)BH);
-  kern<<<grid, C::kThreads, C::kTotal, stream>>>(tq, tk, tv, p);
+  dim3 grid((unsigned)((g->S + kQT - 1) / kQT), (unsigned)BH);
+  kern<<<grid, kThreads, kTotal, stream>>>(tq, tk, tv, p);
   count_launch();
   return check_launch("attn6_kernel");
 }
 
 }  // namespace a6
 
-int launch_attn6(const ea_attn_args* g, int poly, cudaStream_t stream) {
-  const bool trunc = (g->variant & 0x800) != 0;  // experimental: P by truncation (PRMT) instead of F2FP round-to-nearest
-  if (g->variant & 0x4000)  // four query tiles x 32-key blocks: built in round 2, DEADLOCKED on its first B200 run (no trap, the
-    // call had to be killed: profiles/r02_attn_4x32_hang.md) - withdrawn; the bit is rejected so that no caller can reach it
-    return fail(EA_ERR_INVALID, "ea_attn_fwd: the 4 x 32 layout (variant bit 0x4000) was withdrawn - it deadlocked on B200");
-  if (g->variant & 0x2000) {  // three query tiles per CTA, 64-key blocks
-    switch (poly) {
-      case 0: return trunc ? a6::launch<0, false, true, 3, 64>(g, stream) : a6::launch<0, false, false, 3, 64>(g, stream);
-      case 1: return a6::launch<1, false, false, 3, 64>(g, stream);
-      case 4: return trunc ? a6::launch<1, false, true, 3, 64, 8>(g, stream) : a6::launch<1, false, false, 3, 64, 8>(g, stream);    // 1 of 8
-      case 7: return trunc ? a6::launch<1, false, true, 3, 64, 16>(g, stream) : a6::launch<1, false, false, 3, 64, 16>(g, stream);  // 1 of 16
-      default: return fail(EA_ERR_INVALID, "ea_attn_fwd: the 3 x 64 layout takes polynomial code 0, 1 (1 of 4 pairs), 4 (1 of 8) or 7 (1 of 16)");
-    }
-  }
-  switch (poly) {
-    case 0: return trunc ? a6::launch<0, false, true>(g, stream) : a6::launch<0, false, false>(g, stream);
-    case 1: return trunc ? a6::launch<1, false, true>(g, stream) : a6::launch<1, false, false>(g, stream);
-    case 2: return trunc ? a6::launch<2, false, true>(g, stream) : a6::launch<2, false, false>(g, stream);
-    case 3: return a6::launch<3, false, false>(g, stream);
-    case 5: return a6::launch<1, true, false>(g, stream);  // polynomial pairs first, then the MUFU pairs (two phases)
-    case 6: return a6::launch<2, true, false>(g, stream);
-    default: return fail(EA_ERR_INVALID, "ea_attn_fwd: unsupported polynomial fraction (0..3 of every 4 pairs; 5, 6: phased 1, 2)");
-  }
+// One kernel on sm_90a: the exponential-split (bits 4-6), truncated-P (0x800) and three-tile layout (0x2000) selections of
+// ea_attn_args.variant are accepted and all run it.
+int launch_attn6(const ea_attn_args* g, cudaStream_t stream) {
+  return a6::launch(g, stream);
 }
 
 }  // namespace ea

@@ -1,25 +1,18 @@
 #!/usr/bin/env bash
-# Builds libea_b200.so (sm_100a only) in-tree next to the sources' package: easyanimate_b200/libea_b200.so
-#   EA_ATTN_AB=1  also links the retired attention generations of tools/attn_ab/ (A/B measurements only)
+# Builds libea_b200.so (sm_90a, H100) in-tree next to the sources' package: easyanimate_b200/libea_b200.so
 set -euo pipefail
 HERE="$(cd "$(dirname "${BASH_SOURCE[0]}")" && pwd)"
 OUT="$HERE/../libea_b200.so"
 OBJ="$HERE/../_build"
 mkdir -p "$OBJ"
 NVCC="${NVCC:-/usr/local/cuda/bin/nvcc}"
-FLAGS=(-gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -lineinfo -Xcompiler -fPIC --expt-relaxed-constexpr
-       -Xptxas -v -I"$HERE/../../include")
-SRCS=("$HERE"/*.cu)
-AB="${EA_ATTN_AB:-0}"
-if [[ "$AB" == "1" ]]; then
-  FLAGS+=(-DEA_ATTN_AB)
-  SRCS+=("$HERE"/../../tools/attn_ab/*.cu)
-fi
-# a change of the A/B setting invalidates the dispatcher object
-if [[ ! -f "$OBJ/.ab" || "$(cat "$OBJ/.ab")" != "$AB" ]]; then rm -f "$OBJ/attn_api.o"; echo "$AB" > "$OBJ/.ab"; fi
+ARCH=(-gencode arch=compute_90a,code=sm_90a)
+FLAGS=("${ARCH[@]}" -O3 -std=c++17 -lineinfo -Xcompiler -fPIC --expt-relaxed-constexpr -Xptxas -v -I"$HERE/../../include")
+# objects of an earlier build for another architecture are rebuilt
+if [[ ! -f "$OBJ/.arch" || "$(cat "$OBJ/.arch")" != "${ARCH[*]}" ]]; then rm -f "$OBJ"/*.o; echo "${ARCH[*]}" > "$OBJ/.arch"; fi
 pids=()
 objs=()
-for src in "${SRCS[@]}"; do
+for src in "$HERE"/*.cu; do
   obj="$OBJ/$(basename "${src%.cu}").o"
   objs+=("$obj")
   if [[ ! -f "$obj" || "$src" -nt "$obj" || "$HERE/common.cuh" -nt "$obj" || "$HERE/host.h" -nt "$obj" || "$HERE/../../include/ea_b200.h" -nt "$obj" ]]; then
@@ -28,5 +21,5 @@ for src in "${SRCS[@]}"; do
   fi
 done
 for p in "${pids[@]:-}"; do [[ -n "$p" ]] && wait "$p"; done
-"$NVCC" -gencode arch=compute_100a,code=sm_100a -shared -o "$OUT" "${objs[@]}" -lcudart_static -ldl -lrt -lpthread
+"$NVCC" "${ARCH[@]}" -shared -o "$OUT" "${objs[@]}" -lcudart_static -ldl -lrt -lpthread
 echo "built $OUT"

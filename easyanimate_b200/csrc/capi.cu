@@ -39,7 +39,7 @@ extern "C" int ea_enable_peer_access(int32_t peer_device) {
 // CUDA IPC import for the sequence-parallel peer buffers.  The mapping must be made with the IMPORTING kernel's device current
 // (cudaIpcMemLazyEnablePeerAccess then sets up peer access from it to the exporting device): a mapping opened under the
 // exporter's device index - what torch's own storage sharing does - is readable by copy engines but faults when a kernel
-// of another device dereferences it (profiles/r02_debug_sp_ipc.log).
+// of another device dereferences it.
 // Export side: the 64-byte handle of the device allocation that contains `ptr` (cuMemGetAddressRange finds its base; torch's
 // caching allocator sub-allocates from cudaMalloc'ed segments) and ptr's byte offset inside it.
 extern "C" int ea_ipc_export(const void* ptr, void* handle64_out, int64_t* offset_out) {

@@ -1,23 +1,18 @@
-// Causal 3x3x3 (and 1x3x3-free) convolution of the MagViT VAE decoder as an im2col-free implicit GEMM on tcgen05.
+// Causal 3x3x3 convolution of the MagViT VAE as an im2col-free implicit GEMM on sm_90a wgmma.
 //
 // Replaces CausalConv3d.forward (easyanimate/vae/ldm/modules/vaemodules/common.py:84-141, called from
-// ResidualBlock3D common.py:298-323, the upsamplers upsamplers.py:34-37,142-153 and Decoder.conv_in/conv_out
-// omnigen_enc_dec.py:555-615).  The reference runs it one latent frame at a time with a 2-frame cache
-// (padding_flag 3/4); that is one causal convolution over the whole sequence with the first frame replicated on
-// the left, which is what this kernel computes in a single launch per layer.
+// ResidualBlock3D common.py:298-323, the upsamplers upsamplers.py:34-37,142-153, the down-samplers downsamplers.py:24-96
+// and Decoder.conv_in/conv_out omnigen_enc_dec.py:555-615).  The reference runs it one latent frame at a time with a
+// 2-frame cache (padding_flag 3/4); that is one causal convolution over the whole sequence with the first frame replicated
+// on the left, which is what this kernel computes in a single launch per layer.
 //
 // Layout: activations are channels-last [T,H,W,C] bf16.  For an output tile of TH x TW pixels (= 128 GEMM rows) of
 // frame t and every tap (kt,kh,kw) x 64-channel slice, ONE TMA box {64ch, TW, TH, 1} of the input at
 // (w0+kw-1, h0+kh-1, max(t+kt-2,0)) lands in shared memory as a SWIZZLE_128B K-major [128 x 64] A tile - spatial
 // zero padding is TMA out-of-bounds fill, causal replicate padding is the coordinate clamp; nothing is gathered or
-// materialised.  Weights are pre-arranged [Cout, 27*Cin] (tap-major K).  MMA/TMEM/epilogue structure as gemm_tc.cu.
+// materialised.  Weights are pre-arranged [Cout, 27*Cin] (tap-major K).  Warpgroup / barrier / epilogue-staging structure
+// as gemm_tc.cu: one TMA producer thread, two consumer warpgroups of 64 pixels x BN output channels each.
 // Fused in the epilogue: bias, residual add, nearest temporal x2 duplication (frames >= 1), planar NCTHW store.
-// MT = number of 128-pixel sub-tiles one CTA accumulates against the same weight tile (2 => 256x BN CTA tile: the
-// kernel is L2->SM bandwidth bound at 128x128 (64 FLOP/B, ncu: 14.2 TB/s xbar), 256x128 moves 85 FLOP/B).
-// PAIR = CTA pairs (tcgen05 cta_group::2, see gemm_tc.cu): the two CTAs of a cluster take vertically adjacent pixel
-// tiles against the SAME weight tile, each loads half of it, the leader issues M=256 MMAs over both: 256 output
-// channels per pass for the wide layers (BN=256, MT=1: 32 KB per k-block and CTA instead of 48) and 40 KB instead of 48
-// for the 128-channel layers (BN=128, MT=2).
 #include "common.cuh"
 #include "host.h"
 #include "../../include/ea_b200.h"
@@ -26,7 +21,8 @@ namespace ea {
 
 extern void count_launch();
 
-constexpr int kConvThreads = 256;
+constexpr int kConvThreads = 384;
+constexpr int kConvPitch = 132;  // fp32 staging row pitch
 constexpr int kCM = 128;
 constexpr int kCK = 64;
 
@@ -45,41 +41,90 @@ struct ConvDevArgs {
   int st, shw;  // temporal / spatial stride (1 or 2): T, H, W above are the OUTPUT extents (see ea_conv3d_args.stride_*)
 };
 
-template <int BN, int MT, bool PAIR = false>
+template <int BN>
 struct ConvCfg {
-  static constexpr int kABytes = MT * kCM * kCK * 2;
-  static constexpr int kBBytes = (PAIR ? BN / 2 : BN) * kCK * 2;  // PAIR: this CTA's half of the weight tile
+  static constexpr int kABytes = kCM * kCK * 2;
+  static constexpr int kBBytes = BN * kCK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kStages = (200 * 1024) / kStageBytes > 8 ? 8 : (200 * 1024) / kStageBytes;
-  static constexpr int kAccCols = MT * BN;                       // one accumulator stage
-  static constexpr int kTmemCols = 2 * kAccCols < 32 ? 32 : 2 * kAccCols;  // power of two for the shapes used
-  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 + 256;
-  static_assert(kTmemCols <= 512, "accumulators exceed TMEM");
+  static constexpr int kStages = (150 * 1024) / kStageBytes > 8 ? 8 : (150 * 1024) / kStageBytes;
+  static constexpr int kCW = BN < 128 ? BN : 128;  // columns staged per epilogue pass
+  static constexpr int kStagingBytes = 2 * 64 * kConvPitch * 4;
+  static constexpr int kSmemBytes = kStages * kStageBytes + kStagingBytes + 1024 + 256;
+  static_assert(kSmemBytes <= 227 * 1024, "shared memory");
 };
 
-template <int BN, int MT, bool PAIR>
+// bias, residual, frame duplication and the channels-last or planar store of 32 output channels of one pixel
+EA_DEVICE void conv_epilogue_chunk(const ConvDevArgs& p, int t, int ho, int w, int col0, float (&x)[32]) {
+  const int t_out = p.dup_frames ? (t == 0 ? 0 : 2 * t - 1) : t;
+  const int ncopies = (p.dup_frames && t > 0) ? 2 : 1;
+  if (p.out_planar) {
+    // conv_out: few real channels, planar [Cout, T_out, H, W] store
+    for (int j = 0; j < 32 && col0 + j < p.Cout; ++j) {
+      const float v = x[j] + __bfloat162float(p.bias[col0 + j]);
+      for (int cpy = 0; cpy < ncopies; ++cpy)
+        p.out[(((int64_t)(col0 + j) * p.T_out + t_out + cpy) * p.Hout + ho) * p.W + w] = __float2bfloat16_rn(v);
+    }
+    return;
+  }
+  {
+    const uint4* bp = reinterpret_cast<const uint4*>(p.bias + col0);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      uint4 b = __ldg(bp + j);
+      float2 f0 = unpack_bf16x2(b.x), f1 = unpack_bf16x2(b.y), f2 = unpack_bf16x2(b.z), f3 = unpack_bf16x2(b.w);
+      x[j * 8 + 0] += f0.x; x[j * 8 + 1] += f0.y; x[j * 8 + 2] += f1.x; x[j * 8 + 3] += f1.y;
+      x[j * 8 + 4] += f2.x; x[j * 8 + 5] += f2.y; x[j * 8 + 6] += f3.x; x[j * 8 + 7] += f3.y;
+    }
+  }
+  if (p.residual != nullptr) {
+    // (conv2(x) + shortcut): the conv output is a bf16 tensor in the reference before the add (common.py:323)
+    const uint4* rp = reinterpret_cast<const uint4*>(p.residual + (((int64_t)t * p.Hout + ho) * p.W + w) * p.Cout + col0);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      uint4 rr = __ldg(rp + j);
+      uint32_t rw[4] = {rr.x, rr.y, rr.z, rr.w};
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        float2 rf = unpack_bf16x2(rw[q]);
+        x[j * 8 + 2 * q] = bf16_round(x[j * 8 + 2 * q]) + rf.x;
+        x[j * 8 + 2 * q + 1] = bf16_round(x[j * 8 + 2 * q + 1]) + rf.y;
+      }
+    }
+  }
+  uint4 o[4];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    o[j].x = pack_bf16x2(x[j * 8 + 0], x[j * 8 + 1]);
+    o[j].y = pack_bf16x2(x[j * 8 + 2], x[j * 8 + 3]);
+    o[j].z = pack_bf16x2(x[j * 8 + 4], x[j * 8 + 5]);
+    o[j].w = pack_bf16x2(x[j * 8 + 6], x[j * 8 + 7]);
+  }
+  for (int cpy = 0; cpy < ncopies; ++cpy) {
+    uint4* op = reinterpret_cast<uint4*>(p.out + ((((int64_t)(t_out + cpy)) * p.Hout + ho) * p.W + w) * p.Cout + col0);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) op[j] = o[j];
+  }
+}
+
+template <int BN>
 __global__ void __launch_bounds__(kConvThreads, 1)
 conv3d_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
                  const ConvDevArgs p) {
-  using Cfg = ConvCfg<BN, MT, PAIR>;
+  using Cfg = ConvCfg<BN>;
   constexpr int kStages = Cfg::kStages;
+  constexpr int kCW = Cfg::kCW;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + kStages * Cfg::kABytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * Cfg::kStageBytes);
+  float* staging = reinterpret_cast<float*>(smem + kStages * Cfg::kStageBytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * Cfg::kStageBytes + Cfg::kStagingBytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + kStages;
-  uint64_t* tfull_bar = bars + 2 * kStages;
-  uint64_t* tempty_bar = bars + 2 * kStages + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * kStages + 4);
 
-  const int warp = threadIdx.x >> 5;
+  const int wg = threadIdx.x >> 7;
   const int lane = threadIdx.x & 31;
-  const int num_tiles = p.T * p.tiles_h * p.tiles_w * p.tiles_n;  // PAIR: p.tiles_h counts PAIRS of CTA tiles
-  const int crank = PAIR ? (int)cluster_ctarank() : 0;
-  const int first_tile = PAIR ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-  const int tile_step = PAIR ? (int)(gridDim.x >> 1) : (int)gridDim.x;
+  const int num_tiles = p.T * p.tiles_h * p.tiles_w * p.tiles_n;
   const int cchunks = p.Cin / kCK;
   const int num_k_blocks = p.kt_taps * 9 * cchunks;
 
@@ -87,40 +132,29 @@ conv3d_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_consta
     tma_prefetch_desc(&tmap_x);
     tma_prefetch_desc(&tmap_w);
     for (int i = 0; i < kStages; ++i) {
-      mbar_init(&full_bar[i], PAIR ? 2 : 1);  // PAIR: the leader's barrier takes both CTAs' producers and bytes
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], PAIR ? 256 : 128);  // PAIR: the leader's barrier takes both CTAs' epilogue threads
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 8);  // lane 0 of each consumer warp
     }
     fence_mbar_init();
   }
-  if (warp == 2) {
-    if (PAIR) tmem_alloc_2sm(tmem_slot, Cfg::kTmemCols);
-    else tmem_alloc(tmem_slot, Cfg::kTmemCols);
-  }
-  tc_fence_before();
   __syncthreads();
-  if (PAIR) cluster_sync();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   auto decode_tile = [&](int tile, int& t, int& h0, int& w0, int& n0) {
     n0 = (tile % p.tiles_n) * BN;
     int r = tile / p.tiles_n;
     w0 = (r % p.tiles_w) * p.TW;
     r /= p.tiles_w;
-    h0 = p.row0 + ((r % p.tiles_h) * (PAIR ? 2 : 1) + crank) * (MT * p.TH);
+    h0 = p.row0 + (r % p.tiles_h) * p.TH;
     t = r / p.tiles_h;
   };
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (wg == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (threadIdx.x == 0) {
       // ===== TMA producer =====
       int stage = 0;
       uint32_t phase = 0;
-      for (int tile = first_tile; tile < num_tiles; tile += tile_step) {
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         int t, h0, w0, n0;
         decode_tile(tile, t, h0, w0, n0);
         for (int kb = 0; kb < num_k_blocks; ++kb) {
@@ -135,160 +169,70 @@ conv3d_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_consta
           const int xw = p.shw == 1 ? w0 + kw - 1 : 2 * w0 + kw;
           const int xh = p.shw == 1 ? h0 + kh - 1 : 2 * h0 + kh;
           mbar_wait(&empty_bar[stage], phase ^ 1);
-          if (PAIR) {
-            const uint32_t lfull = mapa_shared(smem_u32(&full_bar[stage]), 0);
-            mbar_arrive_expect_tx_cluster(lfull, Cfg::kStageBytes);
-            tma_load_4d_2sm(smem_a + stage * Cfg::kABytes, &tmap_x, lfull, c0, xw, xh, tin);
-            tma_load_2d_2sm(smem_b + stage * Cfg::kBBytes, &tmap_w, lfull, tap * p.Cin + c0, n0 + crank * (BN / 2));
-          } else {
-            mbar_arrive_expect_tx(&full_bar[stage], Cfg::kStageBytes);
-            tma_load_4d(smem_a + stage * Cfg::kABytes, &tmap_x, &full_bar[stage], c0, xw, xh, tin);
-            tma_load_2d(smem_b + stage * Cfg::kBBytes, &tmap_w, &full_bar[stage], tap * p.Cin + c0, n0);
-          }
+          mbar_arrive_expect_tx(&full_bar[stage], Cfg::kStageBytes);
+          tma_load_4d(smem_a + stage * Cfg::kABytes, &tmap_x, &full_bar[stage], c0, xw, xh, tin);
+          tma_load_2d(smem_b + stage * Cfg::kBBytes, &tmap_w, &full_bar[stage], tap * p.Cin + c0, n0);
           if (++stage == kStages) { stage = 0; phase ^= 1; }
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0 && crank == 0) {
-      // ===== MMA issuer (PAIR: the leader CTA issues for both) =====
-      constexpr uint32_t idesc = umma_idesc_bf16(PAIR ? 2 * kCM : kCM, BN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int tile = first_tile; tile < num_tiles; tile += tile_step, ++it) {
-        const int as = it & 1;
-        const uint32_t aphase = (it >> 1) & 1;
-        if (PAIR) mbar_wait_cluster(&tempty_bar[as], aphase ^ 1);
-        else mbar_wait(&tempty_bar[as], aphase ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + as * Cfg::kAccCols;
-        for (int kb = 0; kb < num_k_blocks; ++kb) {
-          if (PAIR) mbar_wait_cluster(&full_bar[stage], phase);
-          else mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint64_t bdesc = umma_desc_sw128(smem_u32(smem_b + stage * Cfg::kBBytes));
-#pragma unroll
-          for (int m = 0; m < MT; ++m) {
-            const uint64_t adesc = umma_desc_sw128(smem_u32(smem_a + stage * Cfg::kABytes + m * (kCM * kCK * 2)));
-#pragma unroll
-            for (int k = 0; k < kCK / 16; ++k) {
-              if (PAIR) umma_ss_2sm(tmem_d + m * BN, adesc + 2 * k, bdesc + 2 * k, idesc, (kb | k) != 0);
-              else umma_ss(tmem_d + m * BN, adesc + 2 * k, bdesc + 2 * k, idesc, (kb | k) != 0);
-            }
-          }
-          if (PAIR) {
-            umma_commit_2sm(&empty_bar[stage], 0x3);
-            if (kb == num_k_blocks - 1) umma_commit_2sm(&tfull_bar[as], 0x3);
-          } else {
-            umma_commit(&empty_bar[stage]);
-            if (kb == num_k_blocks - 1) umma_commit(&tfull_bar[as]);
-          }
-          if (++stage == kStages) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp >= 4) {
-    // ===== epilogue: one output pixel per thread =====
-    const int ew = warp - 4;
-    const int r = ew * 32 + lane;
-    const int ph = r / p.TW, pw = r - ph * p.TW;
-    int it = 0;
-    for (int tile = first_tile; tile < num_tiles; tile += tile_step, ++it) {
-      const int as = it & 1;
-      const uint32_t aphase = (it >> 1) & 1;
+  } else {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    // ===== consumers: GEMM rows (pixels) [64 (wg-1), 64 wg) of the tile =====
+    const int cw = wg - 1;
+    const int tid = threadIdx.x & 127;
+    float* stage_buf = staging + cw * 64 * kConvPitch;
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       int t, h0, w0, n0;
       decode_tile(tile, t, h0, w0, n0);
-      mbar_wait(&tfull_bar[as], aphase);
-      tc_fence_after();
-      const int t_out = p.dup_frames ? (t == 0 ? 0 : 2 * t - 1) : t;
-      const int ncopies = (p.dup_frames && t > 0) ? 2 : 1;
-#pragma unroll 1
-      for (int cc = 0; cc < MT * (BN / 32); ++cc) {
-      const int m = cc / (BN / 32), c = cc % (BN / 32);
-      const int h = h0 + m * p.TH + ph, w = w0 + pw;
-      const bool pix_ok = h < p.row0 + p.Hout && w < p.W;
-      const int ho = h - p.row0;
-      const uint32_t trow = tmem_base + (uint32_t(ew * 32) << 16) + as * Cfg::kAccCols + m * BN;
-      {
-        uint32_t acc[32];
-        __syncwarp();  // threads may have diverged on pix_ok / channel bounds in the previous chunk
-        tmem_ld32(trow + c * 32, acc);
-        tmem_ld_wait();
-        const int col0 = n0 + c * 32;
-        if (!pix_ok || col0 >= p.Cout) continue;
-        float x[32];
+      float acc[BN / 2];
+      int prev = -1;
+      for (int kb = 0; kb < num_k_blocks; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint64_t adesc = gmma_desc_sw128(smem_u32(smem_a + stage * Cfg::kABytes + cw * 64 * 128));
+        const uint64_t bdesc = gmma_desc_sw128(smem_u32(smem_b + stage * Cfg::kBBytes));
+        wgmma_fence();
 #pragma unroll
-        for (int j = 0; j < 32; ++j) x[j] = __uint_as_float(acc[j]);
-        if (p.out_planar) {
-          // conv_out: few real channels, planar [Cout, T_out, H, W] store
-          for (int j = 0; j < 32 && col0 + j < p.Cout; ++j) {
-            const float v = x[j] + __bfloat162float(p.bias[col0 + j]);
-            for (int cpy = 0; cpy < ncopies; ++cpy)
-              p.out[(((int64_t)(col0 + j) * p.T_out + t_out + cpy) * p.Hout + ho) * p.W + w] = __float2bfloat16_rn(v);
-          }
-          continue;
-        }
-        {
-          const uint4* bp = reinterpret_cast<const uint4*>(p.bias + col0);
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            uint4 b = __ldg(bp + j);
-            float2 f0 = unpack_bf16x2(b.x), f1 = unpack_bf16x2(b.y), f2 = unpack_bf16x2(b.z), f3 = unpack_bf16x2(b.w);
-            x[j * 8 + 0] += f0.x; x[j * 8 + 1] += f0.y; x[j * 8 + 2] += f1.x; x[j * 8 + 3] += f1.y;
-            x[j * 8 + 4] += f2.x; x[j * 8 + 5] += f2.y; x[j * 8 + 6] += f3.x; x[j * 8 + 7] += f3.y;
-          }
-        }
-        if (p.residual != nullptr) {
-          // (conv2(x) + shortcut): the conv output is a bf16 tensor in the reference before the add (common.py:323)
-          const uint4* rp =
-              reinterpret_cast<const uint4*>(p.residual + (((int64_t)t * p.Hout + ho) * p.W + w) * p.Cout + col0);
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            uint4 rr = __ldg(rp + j);
-            uint32_t rw[4] = {rr.x, rr.y, rr.z, rr.w};
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              float2 rf = unpack_bf16x2(rw[q]);
-              x[j * 8 + 2 * q] = bf16_round(x[j * 8 + 2 * q]) + rf.x;
-              x[j * 8 + 2 * q + 1] = bf16_round(x[j * 8 + 2 * q + 1]) + rf.y;
-            }
-          }
-        }
-        uint4 o[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          o[j].x = pack_bf16x2(x[j * 8 + 0], x[j * 8 + 1]);
-          o[j].y = pack_bf16x2(x[j * 8 + 2], x[j * 8 + 3]);
-          o[j].z = pack_bf16x2(x[j * 8 + 4], x[j * 8 + 5]);
-          o[j].w = pack_bf16x2(x[j * 8 + 6], x[j * 8 + 7]);
-        }
-        for (int cpy = 0; cpy < ncopies; ++cpy) {
-          uint4* op = reinterpret_cast<uint4*>(p.out + ((((int64_t)(t_out + cpy)) * p.Hout + ho) * p.W + w) * p.Cout + col0);
-#pragma unroll
-          for (int j = 0; j < 4; ++j) op[j] = o[j];
-        }
+        for (int k = 0; k < kCK / 16; ++k) wgmma_ss<BN>(acc, adesc + 2 * k, bdesc + 2 * k, (kb | k) != 0);
+        wgmma_commit();
+        wgmma_wait<1>();  // the k-block before this one has been read: release its stage
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == kStages) { stage = 0; phase ^= 1; }
       }
-      }
-      tc_fence_before();
-      if (PAIR) mbar_arrive_cluster(mapa_shared(smem_u32(&tempty_bar[as]), 0));
-      else mbar_arrive(&tempty_bar[as]);
-    }
-  }
+      wgmma_wait<0>();
+      reg_fence<BN / 2>(acc);
+      if (lane == 0) mbar_arrive(&empty_bar[prev]);
 
-  tc_fence_before();
-  __syncthreads();
-  if (PAIR) cluster_sync();  // no CTA leaves while its peer may still signal it or read its shared memory
-  if (warp == 2) {
-    tc_fence_after();
-    if (PAIR) tmem_dealloc_2sm(tmem_base, Cfg::kTmemCols);
-    else tmem_dealloc(tmem_base, Cfg::kTmemCols);
+      // ===== epilogue: one output pixel and 32 channels per thread and item =====
+#pragma unroll
+      for (int cb = 0; cb < BN / kCW; ++cb) {
+        named_bar_sync(1 + cw, 128);  // the previous pass has finished reading the staging buffer
+        stage_acc<kCW>(acc + cb * (kCW / 2), stage_buf, kConvPitch);
+        named_bar_sync(1 + cw, 128);
+#pragma unroll 1
+        for (int i = tid; i < 64 * (kCW / 32); i += 128) {
+          const int r = i & 63, c = i >> 6;
+          const int row = cw * 64 + r;
+          const int h = h0 + row / p.TW, w = w0 + row % p.TW;
+          const int col0 = n0 + cb * kCW + c * 32;
+          if (h >= p.row0 + p.Hout || w >= p.W || col0 >= p.Cout) continue;
+          float x[32];
+          const float* src = stage_buf + r * kConvPitch + c * 32;
+#pragma unroll
+          for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4*>(x + j) = *reinterpret_cast<const float4*>(src + j);
+          conv_epilogue_chunk(p, t, h - p.row0, w, col0, x);
+        }
+      }
+    }
   }
 }
 
-template <int BN, int MT, bool PAIR = false>
+template <int BN>
 static int launch_conv(const ea_conv3d_args* g, cudaStream_t stream) {
-  using Cfg = ConvCfg<BN, MT, PAIR>;
+  using Cfg = ConvCfg<BN>;
   ConvDevArgs p{};
   p.st = g->stride_t == 2 ? 2 : 1;
   p.shw = g->stride_hw == 2 ? 2 : 1;
@@ -301,11 +245,10 @@ static int launch_conv(const ea_conv3d_args* g, cudaStream_t stream) {
   p.Hout = g->out_rows > 0 ? (int)g->out_rows : p.H;
   // tile shape: 8x16 or 4x32 pixels, whichever wastes fewer out-of-range pixels
   auto waste = [&](int th, int tw) {
-    th *= MT * (PAIR ? 2 : 1);
     return (int64_t)((p.Hout + th - 1) / th) * th * ((p.W + tw - 1) / tw) * tw;
   };
   if (waste(4, 32) < waste(8, 16)) { p.TH = 4; p.TW = 32; } else { p.TH = 8; p.TW = 16; }
-  p.tiles_h = (p.Hout + (PAIR ? 2 : 1) * MT * p.TH - 1) / ((PAIR ? 2 : 1) * MT * p.TH);  // PAIR: pairs of CTA tiles
+  p.tiles_h = (p.Hout + p.TH - 1) / p.TH;
   p.tiles_w = (p.W + p.TW - 1) / p.TW;
   p.tiles_n = (int)((g->Cout_pad + BN - 1) / BN);
   p.kt_taps = 3;
@@ -320,9 +263,9 @@ static int launch_conv(const ea_conv3d_args* g, cudaStream_t stream) {
   {
     uint64_t dims[4] = {(uint64_t)g->Cin, (uint64_t)g->W, (uint64_t)g->H, (uint64_t)g->T};
     uint64_t strides[3] = {(uint64_t)g->Cin * 2, (uint64_t)g->W * g->Cin * 2, (uint64_t)g->H * g->W * g->Cin * 2};
-    // MT sub-tiles stacked along H; with a spatial stride the box spans shw x as many input elements, walked with element
-    // stride shw (cuTensorMapEncodeTiled elementStrides): the number of elements that land is still TW x MT*TH
-    uint32_t box[4] = {kCK, (uint32_t)(p.TW * p.shw), (uint32_t)(MT * p.TH * p.shw), 1};
+    // with a spatial stride the box spans shw x as many input elements, walked with element stride shw
+    // (cuTensorMapEncodeTiled elementStrides): the number of elements that land is still TW x TH
+    uint32_t box[4] = {kCK, (uint32_t)(p.TW * p.shw), (uint32_t)(p.TH * p.shw), 1};
     uint32_t estr[4] = {1, (uint32_t)p.shw, (uint32_t)p.shw, 1};
     int rc = make_tmap_bf16(&tx, g->x, 4, dims, strides, box, true, estr);
     if (rc) return rc;
@@ -331,11 +274,11 @@ static int launch_conv(const ea_conv3d_args* g, cudaStream_t stream) {
     const uint64_t K = (uint64_t)27 * g->Cin;
     uint64_t dims[2] = {K, (uint64_t)g->Cout_pad};
     uint64_t strides[1] = {K * 2};
-    uint32_t box[2] = {kCK, (uint32_t)(PAIR ? BN / 2 : BN)};
+    uint32_t box[2] = {kCK, (uint32_t)BN};
     int rc = make_tmap_bf16(&tw, g->w, 2, dims, strides, box, true);
     if (rc) return rc;
   }
-  auto kern = conv3d_tc_kernel<BN, MT, PAIR>;
+  auto kern = conv3d_tc_kernel<BN>;
   static ::ea::PerDeviceFlag attr_flag;
   const int attr_dev = ::ea::current_device();
   if (!attr_flag.get(attr_dev)) {
@@ -345,25 +288,6 @@ static int launch_conv(const ea_conv3d_args* g, cudaStream_t stream) {
   }
   const int64_t num_tiles = (int64_t)p.T * p.tiles_h * p.tiles_w * p.tiles_n;
   if (num_tiles >= (1ll << 31)) return fail(EA_ERR_INVALID, "ea_conv3d: too many tiles");
-  if (PAIR) {
-    const int clusters = (int)(num_tiles < sm_count() / 2 ? num_tiles : sm_count() / 2);
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)(2 * clusters));
-    cfg.blockDim = dim3(kConvThreads);
-    cfg.dynamicSmemBytes = Cfg::kSmemBytes;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, kern, tx, tw, p);
-    if (e != cudaSuccess) return fail(EA_ERR_CUDA, std::string("cudaLaunchKernelEx(conv, CTA pairs): ") + cudaGetErrorString(e));
-    count_launch();
-    return check_launch("conv3d_tc_kernel (CTA pairs)");
-  }
   const int grid = (int)(num_tiles < sm_count() ? num_tiles : sm_count());
   kern<<<grid, kConvThreads, Cfg::kSmemBytes, stream>>>(tx, tw, p);
   count_launch();
@@ -372,9 +296,6 @@ static int launch_conv(const ea_conv3d_args* g, cudaStream_t stream) {
 
 }  // namespace ea
 
-namespace ea {
-int launch_conv3d_halo(const ea_conv3d_args* g, cudaStream_t stream);  // conv3d_halo.cu
-}
 using namespace ea;
 
 extern "C" int ea_conv3d_causal(const ea_conv3d_args* g, void* stream_) {
@@ -397,21 +318,9 @@ extern "C" int ea_conv3d_causal(const ea_conv3d_args* g, void* stream_) {
                "duplication / planar output");
     EA_REQUIRE(g->stride_hw != 2 || (g->H >= 2 && g->W >= 2), "ea_conv3d_causal: frame too small for stride 2");
   }
-  // unit stride: one halo tile per (kt, channel slice), taps by descriptor offsets (conv3d_halo.cu; +5..18 % over the
-  // tap-per-box kernel below, profiles/r02_conv_halo_bringup.log); variant bit2 keeps the tap-per-box kernel (A/B)
-  if (g->stride_t != 2 && g->stride_hw != 2 && !(g->variant & 4)) return launch_conv3d_halo(g, stream);
-  const int64_t Ho = g->stride_hw == 2 ? g->H / 2 : g->H, Wo = g->stride_hw == 2 ? g->W / 2 : g->W;
-  const int64_t To = g->stride_t == 2 ? (g->T + 1) / 2 : g->T;
-  // 256-pixel CTA tiles against a <=128-wide weight tile (TMEM: 2 stages x 2 sub-tiles x 128 columns) unless the
-  // frame is too small to fill the SMs with them.
-  const int64_t Hw = g->out_rows > 0 ? g->out_rows : Ho;  // rows actually computed
-  const int64_t tiles256 = To * ((Hw + 15) / 16) * ((Wo + 15) / 16) * ((g->Cout_pad + 127) / 128);
-  const bool big = tiles256 >= 2 * sm_count() && !(g->variant & 1);
-  // CTA pairs (variant bit1 disables them: A/B measurements) once there are at least four waves of pair tiles
-  const bool pairs = big && !(g->variant & 2) && tiles256 >= 8 * sm_count();
-  if (pairs && g->Cout_pad % 256 == 0) return launch_conv<256, 1, true>(g, stream);
-  if (pairs && g->Cout_pad % 128 == 0) return launch_conv<128, 2, true>(g, stream);
-  if (g->Cout_pad % 128 == 0) return big ? launch_conv<128, 2>(g, stream) : launch_conv<128, 1>(g, stream);
-  if (g->Cout_pad % 64 == 0) return big ? launch_conv<64, 2>(g, stream) : launch_conv<64, 1>(g, stream);
-  return big ? launch_conv<32, 2>(g, stream) : launch_conv<32, 1>(g, stream);
+  // (ea_conv3d_args.variant selected B200 tile layouts; every value runs the one kernel below)
+  if (g->Cout_pad % 256 == 0) return launch_conv<256>(g, stream);
+  if (g->Cout_pad % 128 == 0) return launch_conv<128>(g, stream);
+  if (g->Cout_pad % 64 == 0) return launch_conv<64>(g, stream);
+  return launch_conv<32>(g, stream);
 }

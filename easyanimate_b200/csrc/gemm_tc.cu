@@ -1,23 +1,14 @@
-// Persistent, warp-specialised tcgen05 GEMM for sm_100a:  D[M,N] = epi(A[M,K] · W[N,K]^T).
+// Persistent, warp-specialised wgmma GEMM for sm_90a:  D[M,N] = epi(A[M,K] · W[N,K]^T).
 //
-//   warp 0 (1 thread)  : TMA producer — cp.async.bulk.tensor tiles of A (128x64) and W (BNx64) into a
-//                        SWIZZLE_128B shared-memory ring, completion on `full` mbarriers.
-//   warp 1 (1 thread)  : MMA issuer  — tcgen05.mma.cta_group::1.kind::f16 (M=128, N=BN, K=16) x4 per stage,
-//                        accumulating fp32 in TMEM; tcgen05.commit releases the smem slot / publishes the tile.
-//   warp 2             : TMEM allocator (2 accumulator stages so the epilogue of tile i overlaps the MMAs of i+1).
-//   warps 4-7          : epilogue — tcgen05.ld (one accumulator row per thread), fused bias / GELU / gate+residual /
-//                        per-head LayerNorm + RoPE, bf16 stores.
-//
-// Large problems (at least four waves of 128x256 tiles) run as CTA PAIRS (gemm2_tc_kernel, tcgen05 cta_group::2): the
-// two CTAs of a cluster own the upper and lower 128 rows of a 256x256 tile, each loads its 128 rows of A and HALF of
-// the W tile, and the leader's single MMA thread issues M=256 instructions that read both halves of W from both SMs.
-// A 128x256 tile per SM pulls 48 KB through the SM's L2 port per 4.2 MFLOP; at the ~55 B/clk/SM that port sustains
-// (14-15 TB/s over 148 SMs, profiles/r01_ncu_conv3d_v1_summary.txt) that is ~1.3 PFLOP/s - what the one-CTA kernel
-// measured.  A plain cluster with TMA multicast of W did not help (the bytes still enter each SM); the pair takes 32 KB.
+//   warpgroup 0 (1 thread) : TMA producer — cp.async.bulk.tensor tiles of A (128x64) and W (BNx64) into a SWIZZLE_128B
+//                            shared-memory ring, completion on `full` mbarriers.
+//   warpgroups 1, 2        : consumers — rows [0,64) / [64,128) of the 128 x BN tile: wgmma.m64nBNk16 (bf16 -> fp32 in
+//                            registers) from both operands in shared memory, then the epilogue: the accumulators go through
+//                            a shared-memory staging buffer so that each thread owns one row of 32 (or 64) consecutive
+//                            columns, fused bias / GELU / gate+residual / per-head LayerNorm + RoPE, bf16 stores.
+// The producer keeps fetching the next tile's k-blocks while the consumers run the epilogue.
 //
 // Replaces the cuBLAS calls behind every nn.Linear of the reference path (see include/ea_b200.h for call sites).
-#include <cstdlib>
-
 #include "common.cuh"
 #include "host.h"
 #include "../../include/ea_b200.h"
@@ -28,7 +19,8 @@ extern void count_launch();
 
 constexpr int kBM = 128;
 constexpr int kBK = 64;
-constexpr int kGemmThreads = 256;
+constexpr int kGemmThreads = 384;
+constexpr int kStagePitch = 132;  // fp32 staging row pitch: conflict-free 16-byte row reads
 
 enum { EPI_QKV = 100 };
 
@@ -68,12 +60,14 @@ struct GemmDevArgs {
 
 template <int BN>
 struct GemmCfg {
-  static constexpr int kStages = BN == 256 ? 4 : (BN == 128 ? 6 : 8);
+  static constexpr int kStages = BN == 256 ? 3 : (BN == 128 ? 4 : 6);
   static constexpr int kABytes = kBM * kBK * 2;
   static constexpr int kBBytes = BN * kBK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kTmemCols = 2 * BN < 32 ? 32 : 2 * BN;  // power of two for BN in {64,128,256}
-  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+  static constexpr int kCW = BN < 128 ? BN : 128;  // columns staged per epilogue pass
+  static constexpr int kStagingBytes = 2 * 64 * kStagePitch * 4;
+  static constexpr int kSmemBytes = kStages * kStageBytes + kStagingBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+  static_assert(kSmemBytes <= 227 * 1024, "shared memory");
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -193,19 +187,10 @@ EA_DEVICE void epilogue_chunk32(const GemmDevArgs& p, int row, int col0, uint32_
 }
 
 // QKV epilogue for one head (64 columns) of one row.
-EA_DEVICE void epilogue_qkv_head(const GemmDevArgs& p, int row, int col0, uint32_t tmem_row_addr) {
-  uint32_t a0[32], a1[32];
-  __syncwarp();  // rows >= M returned early in the previous head
-  tmem_ld32(tmem_row_addr, a0);
-  tmem_ld32(tmem_row_addr + 32, a1);
-  tmem_ld_wait();
-  if (row >= p.M) return;
+EA_DEVICE void epilogue_qkv_head(const GemmDevArgs& p, int row, int col0, const float* src) {
   float x[64];
 #pragma unroll
-  for (int j = 0; j < 32; ++j) {
-    x[j] = __uint_as_float(a0[j]);
-    x[32 + j] = __uint_as_float(a1[j]);
-  }
+  for (int j = 0; j < 64; j += 4) *reinterpret_cast<float4*>(x + j) = *reinterpret_cast<const float4*>(src + j);
   {
     const uint4* bp = reinterpret_cast<const uint4*>(p.bias + col0);
 #pragma unroll
@@ -306,18 +291,17 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
                const GemmDevArgs p) {
   using Cfg = GemmCfg<BN>;
   constexpr int kStages = Cfg::kStages;
+  constexpr int kCW = Cfg::kCW;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + kStages * Cfg::kABytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * Cfg::kStageBytes);
+  float* staging = reinterpret_cast<float*>(smem + kStages * Cfg::kStageBytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * Cfg::kStageBytes + Cfg::kStagingBytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + kStages;
-  uint64_t* tfull_bar = bars + 2 * kStages;
-  uint64_t* tempty_bar = bars + 2 * kStages + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * kStages + 4);
 
-  const int warp = threadIdx.x >> 5;
+  const int wg = threadIdx.x >> 7;
   const int lane = threadIdx.x & 31;
 
   const int num_m_tiles = (p.M + kBM - 1) / kBM;
@@ -330,22 +314,15 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
     tma_prefetch_desc(&tmap_b);
     for (int i = 0; i < kStages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], 128);
+      mbar_init(&empty_bar[i], 8);  // lane 0 of each consumer warp
     }
     fence_mbar_init();
   }
-  if (warp == 2) tmem_alloc(tmem_slot, Cfg::kTmemCols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (wg == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (threadIdx.x == 0) {
       // ===== TMA producer =====
       int stage = 0;
       uint32_t phase = 0;
@@ -361,263 +338,70 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ===== MMA issuer =====
-      constexpr uint32_t idesc = umma_idesc_bf16(kBM, BN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-        const int as = it & 1;
-        const uint32_t aphase = (it >> 1) & 1;
-        mbar_wait(&tempty_bar[as], aphase ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + as * BN;
-        for (int kb = 0; kb < num_k_blocks; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint64_t adesc = umma_desc_sw128(smem_u32(smem_a + stage * Cfg::kABytes));
-          const uint64_t bdesc = umma_desc_sw128(smem_u32(smem_b + stage * Cfg::kBBytes));
-#pragma unroll
-          for (int k = 0; k < kBK / 16; ++k) {
-            // advance 16 bf16 = 32 B inside the 128 B swizzle row: +2 in the (addr >> 4) field
-            umma_ss(tmem_d, adesc + 2 * k, bdesc + 2 * k, idesc, (kb | k) != 0);
-          }
-          umma_commit(&empty_bar[stage]);
-          if (kb == num_k_blocks - 1) umma_commit(&tfull_bar[as]);
-          if (++stage == kStages) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp >= 4) {
-    // ===== epilogue =====
-    const int ew = warp - 4;  // == warp % 4 -> TMEM lanes [32*ew, 32*ew+32)
-    int it = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      const int as = it & 1;
-      const uint32_t aphase = (it >> 1) & 1;
+  } else {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    // ===== consumers: rows [64 (wg-1), 64 wg) of the tile =====
+    const int cw = wg - 1;
+    const int tid = threadIdx.x & 127;
+    float* stage_buf = staging + cw * 64 * kStagePitch;
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int m0 = (tile / num_n_tiles) * kBM;
       const int n0 = (tile % num_n_tiles) * BN;
-      mbar_wait(&tfull_bar[as], aphase);
-      tc_fence_after();
-      const int row = m0 + ew * 32 + lane;
-      const uint32_t trow = tmem_base + (uint32_t(ew * 32) << 16) + as * BN;
-      if constexpr (EPI == EPI_QKV) {
-#pragma unroll 1
-        for (int h = 0; h < BN / 64; ++h) {
-          if (n0 + h * 64 < p.N) epilogue_qkv_head(p, row, n0 + h * 64, trow + h * 64);
-        }
-      } else {
-#pragma unroll 1
-        for (int c = 0; c < BN / 32; ++c) {
-          uint32_t acc[32];
-          __syncwarp();  // reconverge after the masked epilogue of the previous chunk
-          tmem_ld32(trow + c * 32, acc);
-          tmem_ld_wait();
-          if (row < p.M && n0 + c * 32 < p.N) epilogue_chunk32<EPI>(p, row, n0 + c * 32, acc);
-        }
-      }
-      tc_fence_before();
-      mbar_arrive(&tempty_bar[as]);
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::kTmemCols);
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// CTA-pair variant: 256x256 tile per cluster of two, BN = 256 per CTA accumulator (128 rows x 256 fp32 columns, two
-// stages), 6 shared-memory stages of (A 128x64 + W-half 128x64).  Barrier protocol:
-//   full[s]   (leader's, count 2) : both producers arrive.expect_tx on it and both CTAs' TMA bytes complete on it
-//   empty[s]  (each CTA's own)    : the leader's tcgen05.commit multicasts the release to both CTAs
-//   tfull[a]  (each CTA's own)    : multicast commit after the last k-block of a tile
-//   tempty[a] (leader's, count 256): the epilogue threads of BOTH CTAs arrive (the peer's remotely)
-// ------------------------------------------------------------------------------------------------
-struct Gemm2Cfg {
-  static constexpr int kStages = 6;
-  static constexpr int kABytes = kBM * kBK * 2;
-  static constexpr int kBBytes = 128 * kBK * 2;
-  static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kTmemCols = 512;
-  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 + 256;
-};
-
-template <int EPI>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kGemmThreads, 1)
-gemm2_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                const GemmDevArgs p) {
-  using Cfg = Gemm2Cfg;
-  constexpr int BN = 256;
-  constexpr int kStages = Cfg::kStages;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + kStages * Cfg::kABytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * Cfg::kStageBytes);
-  uint64_t* full_bar = bars;
-  uint64_t* empty_bar = bars + kStages;
-  uint64_t* tfull_bar = bars + 2 * kStages;
-  uint64_t* tempty_bar = bars + 2 * kStages + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * kStages + 4);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int crank = (int)cluster_ctarank();
-  const int num_n_tiles = (p.N + BN - 1) / BN;
-  const int num_tiles = ((p.M + 2 * kBM - 1) / (2 * kBM)) * num_n_tiles;  // 256-row tiles
-  const int num_k_blocks = (p.K + kBK - 1) / kBK;
-  const int first_tile = (int)(blockIdx.x >> 1), tile_step = (int)(gridDim.x >> 1);
-
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmap_a);
-    tma_prefetch_desc(&tmap_b);
-    for (int i = 0; i < kStages; ++i) {
-      mbar_init(&full_bar[i], 2);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], 256);
-    }
-    fence_mbar_init();
-  }
-  if (warp == 2) tmem_alloc_2sm(tmem_slot, Cfg::kTmemCols);
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync();  // both CTAs' barriers exist before anything arrives on them remotely
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      // ===== TMA producer (both CTAs): own 128 rows of A, own half of the W tile; completion on the LEADER's barrier =====
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = first_tile; tile < num_tiles; tile += tile_step) {
-        const int m0 = (tile / num_n_tiles) * (2 * kBM) + crank * kBM;
-        const int n0 = (tile % num_n_tiles) * BN + crank * 128;
-        for (int kb = 0; kb < num_k_blocks; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          const uint32_t lfull = mapa_shared(smem_u32(&full_bar[stage]), 0);
-          mbar_arrive_expect_tx_cluster(lfull, Cfg::kStageBytes);
-          tma_load_2d_2sm(smem_a + stage * Cfg::kABytes, &tmap_a, lfull, kb * kBK, m0);
-          tma_load_2d_2sm(smem_b + stage * Cfg::kBBytes, &tmap_b, lfull, kb * kBK, n0);
-          if (++stage == kStages) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0 && crank == 0) {
-      // ===== MMA issuer (leader CTA only) =====
-      constexpr uint32_t idesc = umma_idesc_bf16(2 * kBM, BN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int tile = first_tile; tile < num_tiles; tile += tile_step, ++it) {
-        const int as = it & 1;
-        const uint32_t aphase = (it >> 1) & 1;
-        mbar_wait_cluster(&tempty_bar[as], aphase ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + as * BN;
-        for (int kb = 0; kb < num_k_blocks; ++kb) {
-          mbar_wait_cluster(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint64_t adesc = umma_desc_sw128(smem_u32(smem_a + stage * Cfg::kABytes));
-          const uint64_t bdesc = umma_desc_sw128(smem_u32(smem_b + stage * Cfg::kBBytes));
+      float acc[BN / 2];
+      int prev = -1;
+      for (int kb = 0; kb < num_k_blocks; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint64_t adesc = gmma_desc_sw128(smem_u32(smem_a + stage * Cfg::kABytes + cw * 64 * 128));
+        const uint64_t bdesc = gmma_desc_sw128(smem_u32(smem_b + stage * Cfg::kBBytes));
+        wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < kBK / 16; ++k) umma_ss_2sm(tmem_d, adesc + 2 * k, bdesc + 2 * k, idesc, (kb | k) != 0);
-          umma_commit_2sm(&empty_bar[stage], 0x3);
-          if (kb == num_k_blocks - 1) umma_commit_2sm(&tfull_bar[as], 0x3);
-          if (++stage == kStages) { stage = 0; phase ^= 1; }
+        for (int k = 0; k < kBK / 16; ++k) {
+          // advance 16 bf16 = 32 B inside the 128 B swizzle row: +2 in the (addr >> 4) field
+          wgmma_ss<BN>(acc, adesc + 2 * k, bdesc + 2 * k, (kb | k) != 0);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();  // the k-block before this one has been read: release its stage
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == kStages) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      reg_fence<BN / 2>(acc);
+      if (lane == 0) mbar_arrive(&empty_bar[prev]);
+
+      // ===== epilogue: kCW columns at a time through the staging buffer, one row per thread and column chunk =====
+#pragma unroll
+      for (int cb = 0; cb < BN / kCW; ++cb) {
+        named_bar_sync(1 + cw, 128);  // the previous pass has finished reading the staging buffer
+        stage_acc<kCW>(acc + cb * (kCW / 2), stage_buf, kStagePitch);
+        named_bar_sync(1 + cw, 128);
+        const int c0 = n0 + cb * kCW;
+        if constexpr (EPI == EPI_QKV) {
+#pragma unroll 1
+          for (int i = tid; i < 64 * (kCW / 64); i += 128) {
+            const int r = i & 63, h = i >> 6;
+            const int row = m0 + cw * 64 + r;
+            if (row < p.M && c0 + h * 64 < p.N) epilogue_qkv_head(p, row, c0 + h * 64, stage_buf + r * kStagePitch + h * 64);
+          }
+        } else {
+#pragma unroll 1
+          for (int i = tid; i < 64 * (kCW / 32); i += 128) {
+            const int r = i & 63, c = i >> 6;
+            const int row = m0 + cw * 64 + r;
+            if (row < p.M && c0 + c * 32 < p.N) {
+              uint32_t a32[32];
+              const float* src = stage_buf + r * kStagePitch + c * 32;
+#pragma unroll
+              for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4*>(a32 + j) = *reinterpret_cast<const float4*>(src + j);
+              epilogue_chunk32<EPI>(p, row, c0 + c * 32, a32);
+            }
+          }
         }
       }
     }
-  } else if (warp >= 4) {
-    // ===== epilogue (both CTAs, own 128 rows) =====
-    const int ew = warp - 4;
-    int it = 0;
-    for (int tile = first_tile; tile < num_tiles; tile += tile_step, ++it) {
-      const int as = it & 1;
-      const uint32_t aphase = (it >> 1) & 1;
-      const int m0 = (tile / num_n_tiles) * (2 * kBM) + crank * kBM;
-      const int n0 = (tile % num_n_tiles) * BN;
-      mbar_wait(&tfull_bar[as], aphase);
-      tc_fence_after();
-      const int row = m0 + ew * 32 + lane;
-      const uint32_t trow = tmem_base + (uint32_t(ew * 32) << 16) + as * BN;
-      if constexpr (EPI == EPI_QKV) {
-#pragma unroll 1
-        for (int h = 0; h < BN / 64; ++h) {
-          if (n0 + h * 64 < p.N) epilogue_qkv_head(p, row, n0 + h * 64, trow + h * 64);
-        }
-      } else {
-#pragma unroll 1
-        for (int c = 0; c < BN / 32; ++c) {
-          uint32_t acc[32];
-          __syncwarp();
-          tmem_ld32(trow + c * 32, acc);
-          tmem_ld_wait();
-          if (row < p.M && n0 + c * 32 < p.N) epilogue_chunk32<EPI>(p, row, n0 + c * 32, acc);
-        }
-      }
-      tc_fence_before();
-      mbar_arrive_cluster(mapa_shared(smem_u32(&tempty_bar[as]), 0));
-    }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync();  // no CTA leaves (or frees TMEM) while its peer may still signal it or read its shared memory
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc_2sm(tmem_base, Cfg::kTmemCols);
-  }
-}
-
-template <int EPI>
-static int launch_gemm2(const void* a, int64_t lda, const void* w, int64_t ldw, const GemmDevArgs& p, cudaStream_t stream) {
-  using Cfg = Gemm2Cfg;
-  CUtensorMap ta, tb;
-  {
-    uint64_t dims[2] = {(uint64_t)p.K, (uint64_t)p.M};
-    uint64_t strides[1] = {(uint64_t)lda * 2};
-    uint32_t box[2] = {kBK, kBM};
-    int rc = make_tmap_bf16(&ta, a, 2, dims, strides, box, true);
-    if (rc) return rc;
-  }
-  {
-    uint64_t dims[2] = {(uint64_t)p.K, (uint64_t)p.N};
-    uint64_t strides[1] = {(uint64_t)ldw * 2};
-    uint32_t box[2] = {kBK, 128};
-    int rc = make_tmap_bf16(&tb, w, 2, dims, strides, box, true);
-    if (rc) return rc;
-  }
-  auto kern = gemm2_tc_kernel<EPI>;
-  static ::ea::PerDeviceFlag attr_flag;
-  const int attr_dev = ::ea::current_device();
-  if (!attr_flag.get(attr_dev)) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
-    if (e != cudaSuccess) return fail(EA_ERR_CUDA, std::string("cudaFuncSetAttribute(gemm2): ") + cudaGetErrorString(e));
-    attr_flag.set(attr_dev);
-  }
-  const int num_tiles = ((p.M + 2 * kBM - 1) / (2 * kBM)) * ((p.N + 255) / 256);
-  const int clusters = num_tiles < sm_count() / 2 ? num_tiles : sm_count() / 2;
-  kern<<<2 * clusters, kGemmThreads, Cfg::kSmemBytes, stream>>>(ta, tb, p);
-  count_launch();
-  return check_launch("gemm2_tc_kernel");
-}
-
-// CTA pairs once there are at least four waves of 128x256 tiles (EA_GEMM_2SM=0 disables them: A/B measurements)
-static bool use_pairs(const GemmDevArgs& p) {
-  static const bool enabled = [] { const char* e = getenv("EA_GEMM_2SM"); return !(e && e[0] == '0'); }();
-  // (N a multiple of 256: every shape of the model; ragged widths stay on the one-CTA kernel)
-  return enabled && p.N % 256 == 0 && (int64_t)((p.M + kBM - 1) / kBM) * (p.N / 256) >= 4 * sm_count();
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -664,7 +448,6 @@ static int dispatch_bn(const void* a, int64_t lda, const void* w, int64_t ldw, c
   const int sms = sm_count();
   auto tiles = [&](int bn) { return (int64_t)((p.M + kBM - 1) / kBM) * ((p.N + bn - 1) / bn); };
   // (ragged N is fine for every width: TMA zero-fills the missing weight rows, the epilogue masks the columns)
-  if (use_pairs(p)) return launch_gemm2<EPI>(a, lda, w, ldw, p, stream);
   if (p.N >= 256 && tiles(256) >= sms) return launch_gemm<256, EPI>(a, lda, w, ldw, p, stream);
   if (p.N >= 128 && tiles(128) >= sms / 2) return launch_gemm<128, EPI>(a, lda, w, ldw, p, stream);
   return launch_gemm<64, EPI>(a, lda, w, ldw, p, stream);
@@ -740,7 +523,6 @@ extern "C" int ea_qkv_gemm_ln_rope(const ea_qkv_args* g, void* stream_) {
     }
   }
   // an N tile must not straddle the q|k|v boundaries: the widest tile that divides d
-  if (g->d % 256 == 0 && use_pairs(p)) return launch_gemm2<EPI_QKV>(g->a, g->lda, g->w, g->d, p, stream);
   if (g->d % 256 == 0) return launch_gemm<256, EPI_QKV>(g->a, g->lda, g->w, g->d, p, stream);
   if (g->d % 128 == 0) return launch_gemm<128, EPI_QKV>(g->a, g->lda, g->w, g->d, p, stream);
   return launch_gemm<64, EPI_QKV>(g->a, g->lda, g->w, g->d, p, stream);

@@ -73,11 +73,11 @@ int current_device() {
 int sm_count() {
   static int n[64] = {};
   const int dev = current_device();
-  if (dev < 0 || dev >= 64) return 148;
+  if (dev < 0 || dev >= 64) return 132;
   if (n[dev] == 0) {
     int v = 0;
     cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
-    n[dev] = v > 0 ? v : 148;
+    n[dev] = v > 0 ? v : 132;
   }
   return n[dev];
 }

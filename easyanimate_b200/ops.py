@@ -14,14 +14,10 @@ from . import _lib as L
 
 bf16 = torch.bfloat16
 ATTN_TIMING = None  # set to a list by bench.py to collect (start, end) CUDA events around every attention launch
-# attention kernel selector (include/ea_b200.h `ea_attn_args.variant`): 0x217c = sixth-generation kernel (one TMEM pass,
-# no per-block row maximum on the hot path) in its 3 query tiles x 64-key-block layout with 1 of every 16 column pairs
-# exponentiated by a polynomial on the FMA pipe (the rest on MUFU).  Same box, 47 056 / 13 568 tokens: 2 x 128 layout
-# (0x10c) 890 / 831 TFLOP/s, 3 x 64 all-MUFU (0x210c) 932 / 885 (profiles/r02_attn_microbench_3x64.log); on another box
-# 0x210c 879 / 885, 1 of 8 pairs (0x214c) 885 / 896, 1 of 16 (0x217c) 896 / 921 (profiles/r02_attn_microbench_poly.log).
-# The retired generations exist only in A/B builds (EA_ATTN_AB=1 build.sh).
+# attention kernel selector (include/ea_b200.h `ea_attn_args.variant`); every sixth-generation value runs the one sm_90a
+# attention kernel
 ATTN_VARIANT = int(os.environ.get("EA_ATTN_VARIANT", "0x217c"), 0)
-ATTN_GENERATIONS = L.ea_attn_generations()  # bit 6 always; bits 1, 4, 9 in A/B builds
+ATTN_GENERATIONS = L.ea_attn_generations()  # bit 6
 
 
 def _stream() -> int:

@@ -1,5 +1,5 @@
 """Public sampling API of easyanimate_b200: the denoise loop of ``EasyAnimatePipeline.__call__`` + ``decode_latents``
-(/root/reference/easyanimate/pipeline/pipeline_easyanimate.py:998-1011,1052-1137,722-742) on the B200 modules, for
+(/root/reference/easyanimate/pipeline/pipeline_easyanimate.py:998-1011,1052-1137,722-742) on the H100 modules, for
 callers that do not go through diffusers' ``DiffusionPipeline`` (bench.py, smoke tests, services that feed
 pre-computed text embeddings).  The reference pipelines themselves can be handed
 ``easyanimate_b200.EasyAnimateTransformer3DModel`` / ``AutoencoderKLMagvit`` / ``FlowMatchEulerDiscreteScheduler``

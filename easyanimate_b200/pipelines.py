@@ -1,10 +1,10 @@
-"""The reference's three pipeline entry points with their call signatures, on the B200 modules and WITHOUT diffusers:
+"""The reference's three pipeline entry points with their call signatures, on the H100 modules and WITHOUT diffusers:
 
     EasyAnimatePipeline          easyanimate/pipeline/pipeline_easyanimate.py:175-1148          (predict_t2v.py)
     EasyAnimateInpaintPipeline   easyanimate/pipeline/pipeline_easyanimate_inpaint.py:245-1604  (predict_i2v.py, predict_v2v.py)
     EasyAnimateControlPipeline   easyanimate/pipeline/pipeline_easyanimate_control.py:200-1282  (predict_v2v_control.py)
 
-The reference's own pipeline classes accept the B200 transformer / VAE objects unchanged (INTEGRATION.md section 1, tested by
+The reference's own pipeline classes accept the native transformer / VAE objects unchanged (INTEGRATION.md section 1, tested by
 tests/test_ref_pipeline_cpu.py); these classes are for deployments that do not install diffusers, and they run the loop the
 fused way: per step ONE transformer call on the CFG batch and ONE `ea_cfg_euler_step` (CFG combine + Euler update), frames
 leave the GPU once through `ea_frames_out` (EasyAnimateSampler).  Same keyword arguments, same defaults, same output object
@@ -91,7 +91,7 @@ def add_noise_to_reference_video(image: torch.Tensor, ratio: Optional[float] = N
     return image + torch.where(image == -1, torch.zeros_like(image), noise)
 
 
-class _B200PipelineBase:
+class _NativePipelineBase:
     """Constructor / properties / prompt handling / loop shared by the three pipelines."""
     _callback_tensor_inputs = ["latents", "prompt_embeds", "negative_prompt_embeds", "prompt_embeds_2", "negative_prompt_embeds_2"]
 
@@ -140,7 +140,7 @@ class _B200PipelineBase:
             if m is not None:
                 return m.dtype
         d = self.transformer.dtype
-        return bf16 if d == torch.float8_e4m3fn else d  # fp8 weight STORAGE computes in bf16 (transformer3d.py, DESIGN.md f4)
+        return bf16 if d == torch.float8_e4m3fn else d  # fp8 weight STORAGE computes in bf16 (transformer3d.py)
 
     def to(self, device):
         self.transformer.to(device)
@@ -203,7 +203,7 @@ class _B200PipelineBase:
                      negative_prompt_embeds_2=None, prompt_attention_mask_2=None, negative_prompt_attention_mask_2=None,
                      callback_on_step_end_tensor_inputs=None):
         """The ValueErrors of pipeline_easyanimate.py:600-674, including its insistence on `prompt_embeds_2` when the prompt is
-        given as embeddings (SURVEY.md section 8b: kept so that a call accepted here is accepted there and vice versa)."""
+        given as embeddings."""
         if height % 16 != 0 or width % 16 != 0:
             raise ValueError(f"`height` and `width` have to be divisible by 8 but are {height} and {width}.")
         bad = [k for k in (callback_on_step_end_tensor_inputs or []) if k not in self._callback_tensor_inputs]
@@ -349,7 +349,7 @@ class _B200PipelineBase:
         return len(prompt) if isinstance(prompt, list) else prompt_embeds.shape[0]
 
 
-class EasyAnimatePipeline(_B200PipelineBase):
+class EasyAnimatePipeline(_NativePipelineBase):
     """Text-to-video: pipeline_easyanimate.py:769-1148."""
 
     @torch.no_grad()
@@ -385,7 +385,7 @@ class EasyAnimatePipeline(_B200PipelineBase):
         return self._finish(latents, output_type, return_dict)
 
 
-class EasyAnimateInpaintPipeline(_B200PipelineBase):
+class EasyAnimateInpaintPipeline(_NativePipelineBase):
     """Image-to-video / video-to-video with the InP transformer (33 input channels = 16 latent + 1 mask + 16 masked-video
     latents): pipeline_easyanimate_inpaint.py:978-1604."""
 
@@ -477,7 +477,7 @@ class EasyAnimateInpaintPipeline(_B200PipelineBase):
         return self._finish(latents, output_type, return_dict)
 
 
-class EasyAnimateControlPipeline(_B200PipelineBase):
+class EasyAnimateControlPipeline(_NativePipelineBase):
     """Control (pose / depth / canny video, camera trajectories, reference image): pipeline_easyanimate_control.py:833-1282."""
 
     @torch.no_grad()

@@ -1,6 +1,6 @@
 """Sequence parallelism for ONE video across the ranks of a group.  The reference has no multi-GPU inference code at this
-commit (SURVEY.md section 2.3: no xfuser / ulysses / ring); joint text+video attention (processor.py:287-289) makes a
-per-block exchange unavoidable once one video spans more than the two CFG branches (SURVEY.md section 8e), and this module
+commit; joint text+video attention (processor.py:287-289) makes a
+per-block exchange unavoidable once one video spans more than the two CFG branches, and this module
 is this framework's own design for it (Ulysses-style): every rank owns a contiguous slice of the video tokens for the
 per-token work (AdaLN, projections, feed-forward) and, inside attention, all tokens of a slice of the HEADS.  The text
 tokens are few (256) and replicated.
@@ -11,7 +11,7 @@ Two implementations of the two exchanges per block:
   [B, H/P, S, 64] and the attention-output buffers of every rank are mapped into every other rank (CUDA IPC); the QKV
   projection's epilogue stores head h of its rows straight into the buffer of the rank that owns h, and the attention
   epilogue stores each token's row straight into the token-major buffer of the rank that owns the token
-  (include/ea_b200.h `ea_qkv_peers` / `ea_attn_peers`: 128-byte NVLink stores issued from the same kernels as the tcgen05
+  (include/ea_b200.h `ea_qkv_peers` / `ea_attn_peers`: 128-byte NVLink stores issued from the same kernels as the wgmma
   tiles).  The only collectives left are two 4-byte all-reduces per block that order the kernels of different GPUs.
 * NCCL collectives (`mode="nccl"`, also what the gloo CPU tests run): two `all_to_all_single` + one `all_gather` per block
   plus the permute copies around them - the baseline the fused path is measured against.

@@ -1,10 +1,10 @@
-"""B200-native drop-in for ``easyanimate.models.transformer3d.EasyAnimateTransformer3DModel`` (v5 / v5.1 MMDiT).
+"""H100-native drop-in for ``easyanimate.models.transformer3d.EasyAnimateTransformer3DModel`` (v5 / v5.1 MMDiT).
 
 Same constructor arguments, ``.config`` surface, ``forward`` signature and ``state_dict`` keys as the reference
 (/root/reference/easyanimate/models/transformer3d.py:1346-1689), so ``EasyAnimatePipeline`` /
 ``EasyAnimateInpaintPipeline`` can be handed this module unchanged.  The nn.Linear / nn.LayerNorm / nn.Conv2d
 objects below only OWN the parameters under the reference's key names; the forward pass never calls them — every
-arithmetic step is a kernel of libea_b200.so (tcgen05 GEMMs with fused epilogues, tcgen05 attention, fused
+arithmetic step is a kernel of libea_b200.so (wgmma GEMMs with fused epilogues, wgmma attention, fused
 LayerNorm/AdaLN kernels).  There is no PyTorch/CPU fallback.
 """
 from __future__ import annotations
@@ -23,7 +23,7 @@ bf16 = torch.bfloat16
 
 
 # ---------------------------------------------------------------------------------------------------------------
-# parameter containers (reference key layout; see SURVEY.md §5 "checkpoint / resume")
+# parameter containers (reference key layout)
 # ---------------------------------------------------------------------------------------------------------------
 class _RMSNormParams(nn.Module):
     def __init__(self, dim: int, eps: float = 1e-6):
@@ -94,7 +94,7 @@ class _TimestepEmbedding(nn.Module):
 
 
 class EasyAnimateDiTBlock(nn.Module):
-    """attention.py:1028-1163 on B200 kernels."""
+    """attention.py:1028-1163 on the H100 kernels."""
 
     def __init__(self, dim, num_attention_heads, attention_head_dim, time_embed_dim, norm_elementwise_affine=True,
                  norm_eps=1e-5, is_mmdit_block=True, ff_inner_dim=None):
@@ -385,8 +385,8 @@ class EasyAnimateTransformer3DModel(nn.Module, ConfigMixinLite):
 
     def set_sequence_parallel_group(self, group):
         """Ulysses sequence parallelism over the ranks of `group` for ONE video.  The reference has NO multi-GPU inference
-        path at this commit (SURVEY.md section 2.3); this is this framework's own answer to the per-block exchange joint
-        attention needs (processor.py:287-289, SURVEY.md section 8e).  Every rank calls forward with the same inputs and
+        path at this commit; this is this framework's own answer to the per-block exchange joint
+        attention needs (processor.py:287-289).  Every rank calls forward with the same inputs and
         gets the full output; video tokens and attention heads must divide by the group size.  None restores
         single-GPU execution."""
         from .sequence_parallel import UlyssesAttention

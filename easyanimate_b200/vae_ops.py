@@ -11,7 +11,7 @@ import torch
 from . import _lib as L
 from .ops import _p, _req, _stream, bf16, gemm
 
-CONV_VARIANT = int(os.environ.get("EA_CONV_VARIANT", "0"), 0)  # A/B bits, include/ea_b200.h ea_conv3d_args.variant (bit2: tap-per-box kernel)
+CONV_VARIANT = int(os.environ.get("EA_CONV_VARIANT", "0"), 0)  # include/ea_b200.h ea_conv3d_args.variant (accepted, one kernel)
 
 
 def conv3d_causal(x: torch.Tensor, w_packed: torch.Tensor, bias: torch.Tensor, cout: int, *,

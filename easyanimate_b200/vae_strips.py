@@ -1,5 +1,4 @@
-"""Exact UNTILED decode of one latent video on several GPUs by horizontal strips (SURVEY.md section 8(e) "VAE decode - by
-spatial strips", section 8(f) rank 3).
+"""Exact UNTILED decode of one latent video on several GPUs by horizontal strips.
 
 The reference offers two decodes: untiled (autoencoder_magvit.py:271-287; the whole frame through the Decoder, per-frame
 GroupNorm statistics and mid-block attention over the WHOLE frame) and `tiled_decode` (:381-448; 16 independent decoder passes

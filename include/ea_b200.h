@@ -1,5 +1,5 @@
 /*
- * libea_b200.so — C ABI of the B200-native (sm_100a) kernels behind EasyAnimateV5.1's sampling hot path.
+ * libea_b200.so — C ABI of the H100-native (sm_90a) kernels behind EasyAnimateV5.1's sampling hot path.
  *
  * The reference (aigc-apps/EasyAnimate @ c2a70d1) is 100 % Python: its "operator interface" for this path is the
  * list of torch library calls made by EasyAnimateTransformer3DModel.forward (easyanimate/models/transformer3d.py:1496-1689),
@@ -37,13 +37,13 @@ int ea_abi_version(void);
 uint64_t ea_launch_count(void);
 
 /* ------------------------------------------------------------------------------------------------------------
- * Dense contraction on tcgen05 tensor cores:  out[M,N] = epilogue(A[M,K] · W[N,K]^T + bias[N])
+ * Dense contraction on wgmma tensor cores:  out[M,N] = epilogue(A[M,K] · W[N,K]^T + bias[N])
  * Replaces every nn.Linear on the path (F.linear -> cuBLAS in the reference): processor.py:244-246,261-263,303-311
  * (q/k/v/out projections), diffusers FeedForward built at attention.py:1082-1100 (net.0.proj, net.2),
  * transformer3d.py:1402-1404 (patch-embed Conv2d == GEMM over 2x2 patches), :1410-1413 (text_proj Linear),
  * :1680 (proj_out); VAE 1x1x1 convs (autoencoder_magvit.py:182,281; common.py:291-294) and the VAE
  * mid-block attention projections (attention_processors.py:105-131).
- * A, W are K-major bf16 (row strides lda/ldw in elements, multiples of 8). fp32 accumulation in TMEM.
+ * A, W are K-major bf16 (row strides lda/ldw in elements, multiples of 8). fp32 accumulation in registers (wgmma).
  * ------------------------------------------------------------------------------------------------------------ */
 enum {
   EA_EPI_BIAS = 0,          /* out = bf16(acc + bias)                                                       */
@@ -76,7 +76,7 @@ int ea_gemm(const ea_gemm_args* args, void* stream);
  * Replaces processor.py:244-285 (to_q/to_k/to_v, view/transpose, norm_q/norm_k, cat, apply_rotary_emb).
  * M = B * rows_per_batch (rows_per_batch = S_text or S_video). d = H*64. */
 /* Sequence parallelism for ONE video over up to EA_MAX_PEERS GPUs of a node (no counterpart in the reference, which has
- * no multi-GPU inference path; SURVEY.md section 8e): the two exchanges joint attention needs per block (processor.py:287-289
+ * no multi-GPU inference path: the two exchanges joint attention needs per block (processor.py:287-289
  * sees every token of every head) are FUSED into the kernels on either side of it.  Each GPU projects q/k/v for its slice
  * of the video tokens and all heads; head h of those rows is stored by the projection's epilogue directly into the q/k/v
  * buffer [B, heads_per_peer, S, 64] of the GPU that owns head h (entry h / heads_per_peer: this GPU's own buffer or a
@@ -198,17 +198,10 @@ int ea_dequant_e4m3(const void* w8, void* w16, int64_t n, void* stream);
  * Replaces F.scaled_dot_product_attention + transpose/reshape/split at processor.py:287-303.
  * q,k,v: [B,H,S,64] bf16 contiguous.  Output is token-major and split at S_text:
  * out_text[B,S_text,H*64], out_video[B,S-S_text,H*64].
- * variant selects the kernel (all produce the same softmax):
- *   0x10c: sixth generation - two query tiles per CTA, 128-key blocks, one TMEM pass, exponentials against
- *     the reference kept from earlier key blocks with an end-of-block overflow verdict instead of a per-block row
- *     maximum; bits 4-6: 0-3 = that many of every 4 column pairs by a polynomial on the FMA pipe instead of MUFU,
- *     5/6 = 1/2 of 4 in two phases; bit11 (0x800): P packed by truncation instead of round-to-nearest;
- *     bit13 (0x2000): three query tiles per CTA and 64-key blocks (three softmax warps per SM sub-partition); there the
- *     polynomial code 4 / 7 means 1 of every 8 / 16 pairs - 0x217c is the Python layer's default;
- *     bit14 (0x4000): rejected (a four-tile x 32-key layout, withdrawn after it deadlocked on B200).
- *   Other values select retired generations (first: bits 0-1, fourth: 0x0c|poly<<4, ninth: 0x1000|...), present only in an
- *   A/B build (EA_ATTN_AB=1 build.sh; tools/attn_ab/); ea_attn_generations() returns the bitmask of generations built
- *   in (bit 6 always).  Anything else is EA_ERR_INVALID. */
+ * variant: kept for ABI compatibility.  Any value with (variant & 0x1100) == 0x100 (the sixth-generation codes 0x1?c, 0x2?c,
+ * 0x9?c, ...; the Python layer passes 0x217c) runs the one kernel: a 128-row query tile per CTA, 128-key blocks, wgmma for
+ * Q K^T and P V, online softmax in registers, P rounded to bf16.  The remaining bits no longer select anything.  Other values
+ * are EA_ERR_INVALID; ea_attn_generations() returns 1 << 6. */
 /* The return half of the exchange, fused into the attention epilogue: this GPU ran attention for heads
  * [head0, head0 + H) of out_heads over ALL S tokens; the row of video token v goes into out_video[v / tokens_per_peer]
  * (the token-major [B, tokens_per_peer, out_heads*64] buffer of the GPU that owns the token), text rows into the
@@ -253,7 +246,7 @@ int ea_ipc_close(void* base);
  * ------------------------------------------------------------------------------------------------------------ */
 
 /* Whole-sequence causal 3x3x3 convolution (CausalConv3d.forward, vaemodules/common.py:84-141; temporal left
- * replicate padding 2, spatial zero padding 1) as an implicit GEMM on tcgen05.
+ * replicate padding 2, spatial zero padding 1) as an implicit GEMM on wgmma.
  *   x   [T,H,W,Cin]  bf16, Cin % 64 == 0
  *   w   [Cout_pad, 27*Cin] bf16, k = ((kt*3+kh)*3+kw)*Cin + ci  (rows >= Cout are zero)
  *   out [T',H,W,Cout] channels-last, or planar [Cout,T',H,W] when out_planar (conv_out);
@@ -268,16 +261,14 @@ typedef struct {
   int64_t T, H, W, Cin, Cout, Cout_pad;
   int32_t dup_frames;
   int32_t out_planar;
-  int32_t variant;      /* 0 = default tiling; bit0: force 128-pixel CTA tiles, bit1: no CTA pairs (A/B measurements);
-                         * bit2: tap-per-box kernel for unit-stride calls too (default: halo-tile kernel - one shared-memory
-                         * halo tile per (kt, channel slice), the nine spatial taps by descriptor offsets); bit4: the other
-                         * halo pitch (A/B) */
+  int32_t variant;      /* historical tiling codes, accepted and ignored: every call runs the one sm_90a kernel (a TMA
+                         * box of 128 pixels per tap and 64-channel slice, wgmma into 64 x Cout_tile register tiles) */
   /* Encoder down-sampling convolutions (downsamplers.py:24-96: F.pad(x, (0,1,0,1)) then CausalConv3d(stride=(s_t,2,2),
    * padding 0)): stride_hw = 2 -> out[t,i,j] reads input rows 2i..2i+2 / columns 2j..2j+2 (zeros past the bottom / right
    * edge), out is [T', H/2, W/2, Cout]; stride_t = 2 -> out frame t reads input frames 2t-2..2t (clamped at 0), T' = (T+1)/2.
    * 0 or 1 = unit stride.  Strided calls take no residual / dup_frames / out_planar. */
   int32_t stride_t, stride_hw;
-  /* Output row window (strip-parallel decode, SURVEY.md section 8(e) "by spatial strips"): out_rows > 0 -> only output rows
+  /* Output row window (strip-parallel decode): out_rows > 0 -> only output rows
    * [out_row0, out_row0 + out_rows) of the H input rows are computed and `out` / `residual` are [T', out_rows, W, Cout]
    * (planar: [Cout, T', out_rows, W]); the input then carries its neighbours' halo rows (or zeros at the frame edge) above
    * and below the window.  0 = all rows.  Unit stride only. */
@@ -306,7 +297,7 @@ size_t ea_groupnorm_workspace(int64_t frames, int64_t rows, int64_t groups);
 int ea_groupnorm_stats(const void* x, void* stats, void* workspace, size_t workspace_bytes, int64_t frames, int64_t rows,
                        int64_t W, int64_t C, int64_t groups, float eps, void* stream);
 /* y = [SiLU](bf16((x-mean)*rstd*gamma+beta)) */
-/* Strip-parallel decode (one frame sequence split into row strips over several GPUs, SURVEY.md section 8(e)): the per-frame
+/* Strip-parallel decode (one frame sequence split into row strips over several GPUs): the per-frame
  * GroupNorm statistics are global, so each GPU reduces ITS rows to (sum, sum of squares) per (frame, group) in fp64
  * [frames, groups, 2] (ea_groupnorm_sums; workspace as ea_groupnorm_stats), the pairs of all GPUs are gathered
  * [parts, frames, groups, 2] and added in rank order into the same mean / rstd on every GPU (ea_groupnorm_finalize; count =

@@ -304,7 +304,7 @@ class OracleTeaCache:
 
 def sincos_pos_embed_2d(embed_dim, grid_size, base_size=16):
     """diffusers 0.30/0.31 `get_2d_sincos_pos_embed(embed_dim, (H, W))` restated from its published algorithm (third-party,
-    unpinned - DESIGN.md section 4): numpy float64 [H*W, embed_dim]."""
+    unpinned): numpy float64 [H*W, embed_dim]."""
     def one_d(dim, pos):
         omega = 1.0 / 10000 ** (np.arange(dim // 2, dtype=np.float64) / (dim / 2.0))
         out = np.einsum("m,d->md", pos.reshape(-1), omega)
@@ -488,7 +488,7 @@ def denoise_loop(model: OracleTransformer3D, latents, prompt_embeds, negative_pr
 
 
 def init_weights_(module: nn.Module, seed: int = 1234, std: float = 0.02):
-    """SURVEY.md §8(c)/(d) synthetic init: weights ~N(0,std), norm weights 1+N(0,std), biases N(0,std); AdaLN linears
+    """Synthetic init: weights ~N(0,std), norm weights 1+N(0,std), biases N(0,std); AdaLN linears
     larger (std 0.1) so gates/scales exercise every branch."""
     g = torch.Generator().manual_seed(seed)
     with torch.no_grad():

@@ -5,7 +5,7 @@ get_3d_rotary_pos_embed, randn_tensor; everything else a placeholder).
 
 Two uses:
   * tests/test_ref_pipeline_cpu.py drives `EasyAnimatePipeline.__call__` with the PRODUCT modules plugged in (the boundary of
-    SURVEY.md section 8b: the duck-typed nn.Module surface) and with the reference's own modules, and compares the two;
+    the duck-typed nn.Module surface) and with the reference's own modules, and compares the two;
   * tests/golden/make_golden.py mints `pipe_ref_t2v.safetensors` (latents in, text embeds in, frames out) from the reference's
     pipeline + the reference's transformer and VAE, which the GPU test of the sampler compares with.
 

@@ -1,5 +1,5 @@
 """ORACLE (test infrastructure only) — CPU restatement of AutoencoderKLMagvit.decode (and, as preparation for the I2V
-conditioning row of SURVEY.md §8(f), .encode) for EasyAnimateV5.1.
+conditioning, .encode) for EasyAnimateV5.1.
 
 Only ``tests/``, ``__graft_entry__.smoke()`` and ``bench.py``'s cpu_baseline / ``--impl reference`` legs may import
 this module; it is the checker, never the product path.

@@ -9,10 +9,10 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
-GPU_TEST_TIMEOUT_S = 180  # the longest GPU test takes ~10 s on a B200; a kernel that never returns must not hold the box
+GPU_TEST_TIMEOUT_S = 180  # the longest GPU test takes seconds; a kernel that never returns must not hold the GPU
 
 
 def pytest_collection_modifyitems(config, items):
@@ -20,7 +20,7 @@ def pytest_collection_modifyitems(config, items):
 
     if torch.cuda.is_available():
         # watchdog (pytest-timeout, thread method: dumps the stacks and os._exit()s - a blocked cudaStreamSynchronize cannot be
-        # interrupted by a signal): a deadlocked kernel once held a GPU box for 25 minutes (profiles/r02_attn_4x32_hang.md)
+        # interrupted by a signal)
         if config.pluginmanager.hasplugin("timeout"):
             for item in items:
                 if "gpu" in item.keywords and item.get_closest_marker("timeout") is None:

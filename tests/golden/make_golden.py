@@ -81,9 +81,11 @@ def make_vae_tiled():
         tiled = ref.decode(z).sample
         ref.use_tiling = False
         full = ref.decode(z).sample
-    save_file({"z": z, "out_tiled": tiled.contiguous(), "out_untiled": full.contiguous()}, os.path.join(HERE, "vae_ref_tiled.safetensors"),
-              metadata={"source": "reference AutoencoderKLMagvit.decode (tiled_decode and untiled, fp32, CPU)", "seed": str(seed),
-                        "block_out_channels": str(boc), "tile_sample_min_size": "64"})
+    meta = {"source": "reference AutoencoderKLMagvit.decode (tiled_decode and untiled, fp32, CPU)", "seed": str(seed),
+            "block_out_channels": str(boc), "tile_sample_min_size": "64"}
+    # two files, each under 1 MB
+    save_file({"z": z, "out_tiled": tiled.contiguous()}, os.path.join(HERE, "vae_ref_tiled.safetensors"), metadata=meta)
+    save_file({"out_untiled": full.contiguous()}, os.path.join(HERE, "vae_ref_tiled_2.safetensors"), metadata=meta)
     print("vae_ref_tiled", tuple(tiled.shape), float((tiled - full).abs().max()))
 
 
@@ -233,12 +235,14 @@ def make_pipeline_reference():
                                   num_inference_steps=4, guidance_scale=6.0)
         t[f"z_{tag}"], t[f"frames_{tag}"] = seen["z"].contiguous(), frames.contiguous()
         print("pipe_ref_t2v", tag, tuple(frames.shape), float(frames.mean()), float(seen["z"].float().std()))
-    save_file(t, os.path.join(HERE, "pipe_ref_t2v.safetensors"),
-              metadata={"source": "reference EasyAnimatePipeline.__call__ + reference transformer + reference AutoencoderKLMagvit "
+    meta = {"source": "reference EasyAnimatePipeline.__call__ + reference transformer + reference AutoencoderKLMagvit "
                                   "(CPU; diffusers names from oracle/_refshim: FlowMatchEulerDiscreteScheduler shift=1, "
                                   "get_3d_rotary_pos_embed)", "config": repr(PIPE_CFG), "block_out_channels": repr(PIPE_BOC),
                         "steps": "4", "guidance_scale": "6.0", "height": "64", "width": "96", "video_length": "9",
-                        "seeds": "transformer 41, vae 42, inputs 43"})
+                        "seeds": "transformer 41, vae 42, inputs 43"}
+    # two files, each under 1 MB
+    save_file({k: v for k, v in t.items() if k != "frames_fp32"}, os.path.join(HERE, "pipe_ref_t2v.safetensors"), metadata=meta)
+    save_file({"frames_fp32": t["frames_fp32"]}, os.path.join(HERE, "pipe_ref_t2v_2.safetensors"), metadata=meta)
 
 
 TEACACHE_COEFFS = [1.07862322, -4.19362456, 3.06725828, 0.33161686, 0.02374758]  # transformer3d.py:131 (v5.1-7b)

@@ -1,4 +1,4 @@
-"""Three-way parity criterion used by the GPU tests (SURVEY.md §7 'Tolerance vs dtype').
+"""Three-way parity criterion used by the GPU tests.
 
 north_star asks for rtol=1e-3/atol=1e-4 "bf16", which is tighter than one bf16 ulp (2^-8 relative): two *correct*
 bf16 implementations of the same network differ by more than that.  So every module-level test checks

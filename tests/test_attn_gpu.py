@@ -1,15 +1,12 @@
-"""tcgen05 attention kernels against an fp32 PyTorch reference of softmax(QK^T/sqrt(64))V (GPU only)."""
+"""wgmma attention kernel against an fp32 PyTorch reference of softmax(QK^T/sqrt(64))V (GPU only)."""
 import pytest
 import torch
 
 pytestmark = pytest.mark.gpu
 bf16 = torch.bfloat16
 
-# 0x10c: default - sixth generation (two query tiles per CTA, one TMEM pass, optimistic reference / end-of-block verdict,
-# all exponentials on MUFU); 0x11c / 0x12c: 1 / 2 of every 4 column pairs by the FMA-pipe polynomial; 0x15c / 0x16c: the
-# same in two phases; 0x90c: P by truncation; 0x100c-0x104c: ninth generation (tensor-core row sums, 112-key blocks,
-# 0..4 of 8 pairs by polynomial); 0x1c / 0x0c / 0x3c: fourth generation (per-block row maximum); 0-3: first generation
-# (the retired generations are tested only when the library was built with EA_ATTN_AB=1)
+# The variant codes of include/ea_b200.h `ea_attn_args.variant`: every sixth-generation code (0x1?c, 0x2?c, 0x9?c) runs the one
+# sm_90a kernel and must give the same softmax; codes of generations that are not built in are skipped
 def _variants(all_of):
     from easyanimate_b200 import _lib
     gens = _lib.ea_attn_generations()
@@ -65,9 +62,9 @@ def test_attention_large_logits_and_running_max_rescale():
 @pytest.mark.parametrize("variant", _variants([0x10C, 0x11C, 0x13C, 0x15C, 0x90C, 0x210C, 0x211C, 0x214C, 0x217C, 0x100C, 0x101C, 0x102C, 0x1C]))
 @pytest.mark.parametrize("col,mag", [(640, 150.0), (643, 150.0), (640, 1500.0), (643, 1500.0), (130, 40.0), (1023, 800.0), (740, 1500.0), (700, 150.0)])
 def test_attention_outlier_key_beyond_the_kept_reference(variant, col, mag):
-    """One key whose score exceeds everything before it by far more than 2^30 (in a polynomial-exp column, col % 8 < 2,
-    or a MUFU column): the optimistic-reference kernel must notice (row-sum / polynomial-argument guard) and redo the
-    block with the true row maximum; rows anti-aligned with the key see a hugely negative score instead."""
+    """One key whose score exceeds everything before it by far more than 2^30, at several columns of a 128-key block and in
+    a ragged last block: the online softmax must rescale O and the row sum by the new running maximum; rows anti-aligned with
+    the key see a hugely negative score instead."""
     from easyanimate_b200 import ops
     B, H, S = 1, 2, 1100
     g = torch.Generator(device="cuda").manual_seed(11)

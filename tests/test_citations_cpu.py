@@ -1,28 +1,22 @@
 """Every `file.py:NN[-MM]` citation of a reference file in the product, the oracle, the tests and the docs points INSIDE that file
-(VERDICT round 1 found citations of lines that do not exist).  Range check only - what the lines say is the reviewer's job.
-Skipped where /root/reference is absent."""
+Range check only - what the lines say is the reviewer's job.  The line counts of the reference's .py / .yaml / .txt / .toml
+files (per base name) are stored in tests/golden/reference_line_counts.json."""
 import glob
+import json
 import os
 import re
 
-import pytest
-
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference"
-pytestmark = pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "easyanimate")), reason="/root/reference not present")
 PAT = re.compile(r"([A-Za-z0-9_]+\.(?:py|yaml|txt|toml)):(\d+)(?:[-–](\d+))?((?:,\s*\d+(?:[-–]\d+)?)*)")
 
 
 def test_reference_citations_are_inside_the_cited_files():
-    lengths = {}
-    for pat in ("**/*.py", "**/*.yaml", "*.txt", "*.toml"):
-        for p in glob.glob(os.path.join(REF, pat), recursive=True):
-            with open(p, errors="replace") as f:
-                lengths.setdefault(os.path.basename(p), []).append(sum(1 for _ in f))
+    with open(os.path.join(ROOT, "tests", "golden", "reference_line_counts.json")) as f:
+        lengths = json.load(f)
     files = [p for pat in ("easyanimate_b200/**/*.py", "easyanimate_b200/csrc/*.cu*", "easyanimate_b200/csrc/*.h", "include/*.h",
                            "oracle/**/*.py", "tests/**/*.py", "tools/*.py", "*.md", "bench.py", "__graft_entry__.py")
              for p in glob.glob(os.path.join(ROOT, pat), recursive=True)
-             if os.path.basename(p) not in ("VERDICT.md", "SURVEY.md", "BASELINE.md", "PAPERS.md", "SNIPPETS.md", "ADVICE.md")]
+             if os.path.basename(p) not in ("PAPERS.md", "SNIPPETS.md")]
     checked, bad = 0, []
     for path in files:
         with open(path, errors="replace") as f:

@@ -1,8 +1,8 @@
 """Pinning the third-party (`diffusers` 0.30.1-0.31.0) arithmetic the EasyAnimateV5.1 path calls, which oracle/dit.py and
-oracle/_refshim restate because diffusers can be installed neither here nor on the GPU box (VERDICT round 1, weak item 4).
+oracle/_refshim restate because diffusers can be installed neither here nor on the GPU box.
 
-Part A runs wherever /root/reference and `transformers` exist and compares the restatements with INDEPENDENT copies of the same
-published functions that do exist on this box:
+Part A compares the restatements with INDEPENDENT copies of the same published functions (where the reference tree is not
+installed, with the tables those copies produced, tests/golden/diffusers_pin_ref.safetensors, tests/refgold.py):
   * `get_2d_sincos_pos_embed`  <- the reference's own vendored copy (easyanimate/models/patch.py:12-58, diffusers' function with
     interpolation_scale / base_size) and transformers' MAE original (models/vit_mae/modeling_vit_mae.py);
   * `get_timestep_embedding`   <- the reference's vendored DDPM original (easyanimate/vae/ldm/modules/diffusionmodules/model.py:
@@ -12,7 +12,7 @@ published functions that do exist on this box:
 Part B runs only where a real `diffusers` is importable (skipped otherwise - on both boxes of this build) and compares every
 restated primitive with the real class / function: scheduler, 3-D RoPE table, Timesteps, apply_rotary_emb, AdaLayerNorm,
 FeedForward(gelu-approximate), get_2d_sincos_pos_embed.  Until Part B has run somewhere, the scheduler and
-`get_3d_rotary_pos_embed` stay "parity unpinned" (DESIGN.md section 4)."""
+`get_3d_rotary_pos_embed` stay "parity unpinned"."""
 import ast
 import importlib.util
 import math
@@ -24,6 +24,7 @@ import pytest
 import torch
 
 from oracle import dit
+from tests import refgold
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SHIM_DIR = os.path.join(os.path.dirname(HERE), "oracle", "_refshim", "diffusers")
@@ -52,17 +53,34 @@ def _lift(path, names, env):
     return ns
 
 
-needs_ref = pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "easyanimate")), reason="/root/reference not present")
+LIVE = os.path.isdir(os.path.join(REF, "easyanimate"))
+GOLD = refgold.Store("diffusers_pin_ref")
+
+
+@pytest.fixture(scope="module", autouse=True)
+def _save_minted():
+    yield
+    GOLD.save()
+
+
+def _ref_table(key, compute):
+    """The reference's table: computed live where the reference tree exists (recorded when minting), else the stored one."""
+    if LIVE:
+        want = torch.as_tensor(compute())
+        if refgold.MINT:
+            GOLD.tensors[key] = want.contiguous()
+        return want
+    return GOLD.tensors[key]
 
 
 # ---- Part A ---------------------------------------------------------------------------------------------------------
-@needs_ref
 @pytest.mark.parametrize("dim,grid,base", [(128, (4, 6), 16), (256, (8, 8), 8), (64, (5, 3), 16)])
 def test_sincos_2d_table_matches_the_references_vendored_copy(dim, grid, base):
     emb, _ = _shim()
-    ref = _lift(os.path.join(REF, "easyanimate", "models", "patch.py"),
-                ["get_2d_sincos_pos_embed", "get_2d_sincos_pos_embed_from_grid", "get_1d_sincos_pos_embed_from_grid"], {"np": np})
-    want = ref["get_2d_sincos_pos_embed"](dim, grid, base_size=base)
+    want = _ref_table(f"sincos_{dim}_{grid[0]}x{grid[1]}_{base}", lambda: _lift(
+        os.path.join(REF, "easyanimate", "models", "patch.py"),
+        ["get_2d_sincos_pos_embed", "get_2d_sincos_pos_embed_from_grid", "get_1d_sincos_pos_embed_from_grid"],
+        {"np": np})["get_2d_sincos_pos_embed"](dim, grid, base_size=base)).numpy()
     got_shim = emb.get_2d_sincos_pos_embed(dim, grid, base_size=base)
     got_oracle = dit.sincos_pos_embed_2d(dim, grid, base_size=base)
     assert np.array_equal(np.asarray(got_shim), want)
@@ -78,14 +96,13 @@ def test_sincos_2d_table_matches_transformers_mae_original():
         assert np.allclose(np.asarray(got), np.asarray(want), rtol=0, atol=1e-12)
 
 
-@needs_ref
 @pytest.mark.parametrize("dim", [64, 128, 512])
 def test_timestep_embedding_matches_the_references_vendored_ddpm_original(dim):
     emb, _ = _shim()
-    ref = _lift(os.path.join(REF, "easyanimate", "vae", "ldm", "modules", "diffusionmodules", "model.py"),
-                ["get_timestep_embedding"], {"math": math, "torch": torch})
     t = torch.tensor([0.0, 1.0, 421.0, 937.5, 1000.0])
-    want = ref["get_timestep_embedding"](t, dim)
+    want = _ref_table(f"timestep_{dim}", lambda: _lift(
+        os.path.join(REF, "easyanimate", "vae", "ldm", "modules", "diffusionmodules", "model.py"),
+        ["get_timestep_embedding"], {"math": math, "torch": torch})["get_timestep_embedding"](t, dim))
     for f in (emb.get_timestep_embedding, dit.get_timestep_embedding):
         # same formula, different association of the fp32 products (DDPM: arange * (-log/(h-1)); diffusers: (-log * arange)/(h-1)):
         # arguments up to 1000 rad -> 1e-7 relative is ~1e-4 absolute in sin / cos

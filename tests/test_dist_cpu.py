@@ -149,7 +149,7 @@ def _teacache_worker(rank, port, q):
 
 
 def test_teacache_with_cfg_parallel_takes_the_joint_batch_decision():
-    """ADVICE r1 (medium): with cfg_group each rank sees one branch (B=1); the reference decides skip/compute once per step
+    """With cfg_group each rank sees one branch (B=1); the reference decides skip/compute once per step
     from the rel-L1 means over the batch of 2 (transformer3d.py:1563-1586).  The (num, den) sums are all-reduced over the
     CFG pair, so both ranks skip exactly where the single-process batch-of-2 run skips and the latents agree bit for bit."""
     ctx = mp.get_context("spawn")

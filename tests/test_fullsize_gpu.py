@@ -102,8 +102,8 @@ def test_vae_decode_720p_is_causal_in_time():
     from easyanimate_b200 import vae_ops
     saved = vae_ops.CONV_VARIANT
     try:
-        # (1) one kernel family for both decodes (CTA pairs off: with them the 3-frame and the 13-frame decode pick
-        # different tile shapes for some layers, and bit-equality across tensor-core instruction shapes is not promised)
+        # (1) the 3-frame and the 13-frame decode take the same tile shapes for every layer (variant bit 2 of the ABI is
+        # accepted and selects the same kernel)
         vae_ops.CONV_VARIANT = saved | 2
         with torch.no_grad():
             full = vae.decode(z).sample

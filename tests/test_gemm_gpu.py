@@ -1,4 +1,4 @@
-"""tcgen05 GEMM and its fused epilogues against a plain PyTorch fp32 reference of the same op (GPU only)."""
+"""wgmma GEMM and its fused epilogues against a plain PyTorch fp32 reference of the same op (GPU only)."""
 import pytest
 import torch
 

@@ -2,14 +2,17 @@
 against the REFERENCE's own pipeline classes, both over the same product modules with the kernels replaced by the torch
 stand-ins of tests/cpu_ops.py: same inputs, same seeded noise -> the same frames.  What differs between the two runs is only the
 host code under test here (prompt plumbing, latent shapes, noise draw, conditioning preparation, schedule indexing, the fused
-CFG + Euler update instead of four tensor ops, the fused output tail)."""
+CFG + Euler update instead of four tensor ops, the fused output tail).
+Where the reference is not installed the product's frames are compared with a stored sample of the reference's frames
+(tests/golden/native_pipelines_ref.safetensors, tests/refgold.py)."""
 import pytest
 import torch
 
 from oracle import dit, ref_pipeline, vae
-from tests import cpu_ops
+from tests import cpu_ops, refgold
 
-pytestmark = pytest.mark.skipif(not ref_pipeline.available(), reason="/root/reference not present")
+LIVE = ref_pipeline.available()
+GOLD = refgold.Store("native_pipelines_ref")
 bf16 = torch.bfloat16
 CFG = dict(num_attention_heads=2, attention_head_dim=64, in_channels=16, out_channels=16, patch_size=2, num_layers=2,
            time_embed_dim=64, add_norm_text_encoder=True, text_embed_dim=128, text_embed_dim_t5=None,
@@ -63,9 +66,25 @@ def _mask_kw(pe, ne):
                 prompt_embeds_2=pe, prompt_attention_mask_2=ones.clone())
 
 
+@pytest.fixture(scope="module", autouse=True)
+def _save_minted():
+    yield
+    GOLD.save()
+
+
 def _same(a, b):
     assert a.shape == b.shape and a.dtype == b.dtype == torch.float32
     assert torch.equal(a, b), float((a - b).abs().max())
+
+
+def _same_ref(key, got, reference):
+    """got == the frames `reference()` computes with the reference's pipeline class (live), or its stored sample."""
+    assert got.dtype == torch.float32
+    GOLD.same_sample(key, got, reference() if LIVE else None)
+
+
+def _live(fn):
+    return fn if LIVE else None
 
 
 def test_t2v_pipeline_equals_the_reference_pipeline(on_cpu):
@@ -74,29 +93,29 @@ def test_t2v_pipeline_equals_the_reference_pipeline(on_cpu):
     g = torch.Generator().manual_seed(1)
     lat = torch.randn(1, 16, LF, H // 8, W // 8, generator=g).to(bf16)
     pe, ne = _embeds(g)
-    want = ref_pipeline.run(ref_pipeline.reference_pipeline(t, v), lat, pe, ne, height=H, width=W, video_length=FRAMES,
-                            num_inference_steps=STEPS)
     pipe = EasyAnimatePipeline(vae=v, transformer=t)
     out = pipe(video_length=FRAMES, height=H, width=W, num_inference_steps=STEPS, guidance_scale=6.0, latents=lat, **_mask_kw(pe, ne))
-    _same(out.frames, want)
+    _same_ref("t2v", out.frames, lambda: ref_pipeline.run(ref_pipeline.reference_pipeline(t, v), lat, pe, ne, height=H, width=W,
+                                                          video_length=FRAMES, num_inference_steps=STEPS))
     assert pipe.num_timesteps == STEPS and out[0] is out.frames
     # noise drawn by the pipeline itself: the reference's randn_tensor semantics (CPU generator, transformer dtype)
-    want = ref_pipeline.reference_pipeline(t, v)(video_length=FRAMES, height=H, width=W, num_inference_steps=2, guidance_scale=6.0,
-                                                  generator=torch.Generator().manual_seed(5), **_mask_kw(pe, ne)).frames
     got = pipe(video_length=FRAMES, height=H, width=W, num_inference_steps=2, guidance_scale=6.0,
                generator=torch.Generator().manual_seed(5), **_mask_kw(pe, ne), output_type="numpy", return_dict=False)
     assert isinstance(got, __import__("numpy").ndarray)
-    _same(torch.from_numpy(got), want)
+    _same_ref("t2v_generator", torch.from_numpy(got), lambda: ref_pipeline.reference_pipeline(t, v)(
+        video_length=FRAMES, height=H, width=W, num_inference_steps=2, guidance_scale=6.0, generator=torch.Generator().manual_seed(5),
+        **_mask_kw(pe, ne)).frames)
     # no guidance (guidance_scale <= 1): one forward per step, no negative prompt needed
-    want = ref_pipeline.reference_pipeline(t, v)(video_length=FRAMES, height=H, width=W, num_inference_steps=2, guidance_scale=1.0,
-                                                  latents=lat, **_mask_kw(pe, ne)).frames
-    _same(pipe(video_length=FRAMES, height=H, width=W, num_inference_steps=2, guidance_scale=1.0, latents=lat, **_mask_kw(pe, ne)).frames, want)
+    _same_ref("t2v_no_guidance", pipe(video_length=FRAMES, height=H, width=W, num_inference_steps=2, guidance_scale=1.0, latents=lat,
+                                      **_mask_kw(pe, ne)).frames,
+              lambda: ref_pipeline.reference_pipeline(t, v)(video_length=FRAMES, height=H, width=W, num_inference_steps=2,
+                                                            guidance_scale=1.0, latents=lat, **_mask_kw(pe, ne)).frames)
 
 
 def test_t2v_pipeline_rejects_what_the_reference_rejects(on_cpu):
     from easyanimate_b200 import EasyAnimatePipeline
     t, v = _modules(on_cpu)
-    pipe, ref = EasyAnimatePipeline(vae=v, transformer=t), ref_pipeline.reference_pipeline(t, v)
+    pipe = EasyAnimatePipeline(vae=v, transformer=t)
     g = torch.Generator().manual_seed(2)
     pe, ne = _embeds(g)
     ok = dict(video_length=FRAMES, height=H, width=W, num_inference_steps=2, guidance_scale=6.0)
@@ -107,12 +126,16 @@ def test_t2v_pipeline_rejects_what_the_reference_rejects(on_cpu):
         dict(ok, prompt="a cat", **_mask_kw(pe, ne)),                                          # both prompt and embeds
         dict(ok, **_mask_kw(pe, ne), callback_on_step_end_tensor_inputs=["nope"]),
     ]
-    for kw in bad_calls:
+    def ref_message(kw):
         with pytest.raises(ValueError) as e_ref:
-            ref(**kw)
+            ref_pipeline.reference_pipeline(t, v)(**kw)
+        return str(e_ref.value).split(":")[0][:40]
+
+    for i, kw in enumerate(bad_calls):
+        want = GOLD.value(f"rejects_{i}", _live(lambda: ref_message(kw)))
         with pytest.raises(ValueError) as e_ours:
             pipe(**kw)
-        assert str(e_ours.value).split(":")[0][:40] == str(e_ref.value).split(":")[0][:40]
+        assert str(e_ours.value).split(":")[0][:40] == want
     with pytest.raises(NotImplementedError):
         pipe(**ok, **_mask_kw(pe, ne), guidance_rescale=0.7)
 
@@ -126,15 +149,16 @@ def test_callback_on_step_end_sees_and_replaces_latents(on_cpu):
     seen = []
 
     def cb(pipe, i, t_, kw):
-        seen.append((i, float(t_), tuple(kw["latents"].shape)))
+        seen.append([i, float(t_), list(kw["latents"].shape)])
         return {"latents": kw["latents"] * 0.5} if i == 0 else {}
 
     kw = dict(video_length=FRAMES, height=H, width=W, num_inference_steps=STEPS, guidance_scale=6.0, latents=lat, **_mask_kw(pe, ne))
-    want = ref_pipeline.reference_pipeline(t, v)(callback_on_step_end=cb, **kw).frames
-    ref_seen, seen[:] = list(seen), []
+    want = ref_pipeline.reference_pipeline(t, v)(callback_on_step_end=cb, **kw).frames if LIVE else None
+    ref_seen = GOLD.value("callback_seen", _live(lambda: list(seen)))
+    seen[:] = []
     got = EasyAnimatePipeline(vae=v, transformer=t)(callback_on_step_end=cb, **kw).frames
     assert seen == ref_seen and len(seen) == STEPS
-    _same(got, want)
+    _same_ref("callback", got, lambda: want)
 
 
 @pytest.mark.parametrize("strength", [1.0, 0.7])
@@ -149,9 +173,9 @@ def test_inpaint_pipeline_equals_the_reference_pipeline(on_cpu, strength):
     pe, ne = _embeds(g)
     kw = dict(video_length=FRAMES, video=video, mask_video=mask, height=H, width=W, num_inference_steps=4, guidance_scale=6.0,
               strength=strength, noise_aug_strength=0.0563, **_mask_kw(pe, ne))
-    want = ref_pipeline.reference_inpaint_pipeline(t, v)(generator=torch.Generator().manual_seed(9), **kw).frames
     got = EasyAnimateInpaintPipeline(vae=v, transformer=t)(generator=torch.Generator().manual_seed(9), **kw).frames
-    _same(got, want)
+    _same_ref(f"inpaint_{strength}", got,
+              lambda: ref_pipeline.reference_inpaint_pipeline(t, v)(generator=torch.Generator().manual_seed(9), **kw).frames)
 
 
 def test_inpaint_pipeline_all_masked_is_zero_conditioning(on_cpu):
@@ -164,8 +188,8 @@ def test_inpaint_pipeline_all_masked_is_zero_conditioning(on_cpu):
     pe, ne = _embeds(g)
     kw = dict(video_length=FRAMES, video=video, mask_video=mask, height=H, width=W, num_inference_steps=2, guidance_scale=6.0,
               **_mask_kw(pe, ne))
-    want = ref_pipeline.reference_inpaint_pipeline(t, v)(generator=torch.Generator().manual_seed(10), **kw).frames
-    _same(EasyAnimateInpaintPipeline(vae=v, transformer=t)(generator=torch.Generator().manual_seed(10), **kw).frames, want)
+    _same_ref("inpaint_all_masked", EasyAnimateInpaintPipeline(vae=v, transformer=t)(generator=torch.Generator().manual_seed(10), **kw).frames,
+              lambda: ref_pipeline.reference_inpaint_pipeline(t, v)(generator=torch.Generator().manual_seed(10), **kw).frames)
 
 
 @pytest.mark.parametrize("mode", ["control_video+ref", "control_video", "camera", "none"])
@@ -182,8 +206,8 @@ def test_control_pipeline_equals_the_reference_pipeline(on_cpu, mode):
         kw["ref_image"] = torch.rand(1, 3, 1, H, W, generator=g)
     if mode == "camera":
         kw["control_camera_video"] = torch.randn(1, 16, FRAMES, H, W, generator=g)
-    want = ref_pipeline.reference_control_pipeline(t, v)(**kw).frames
-    _same(EasyAnimateControlPipeline(vae=v, transformer=t)(**kw).frames, want)
+    _same_ref(f"control_{mode}", EasyAnimateControlPipeline(vae=v, transformer=t)(**kw).frames,
+              lambda: ref_pipeline.reference_control_pipeline(t, v)(**kw).frames)
 
 
 class _FakeTokens(dict):
@@ -234,18 +258,21 @@ def test_prompt_strings_go_through_the_llm_branch_like_the_reference(on_cpu):
     t, v = _modules(on_cpu)
     torch.manual_seed(0)
     tok, enc = _FakeTokenizer(), _FakeTextEncoder(128).to(bf16)
-    ref = ref_pipeline.reference_pipeline(t, v)
-    ref.tokenizer, ref.text_encoder = tok, enc
+    ref = None
+    if LIVE:
+        ref = ref_pipeline.reference_pipeline(t, v)
+        ref.tokenizer, ref.text_encoder = tok, enc
     lat = torch.randn(1, 16, LF, H // 8, W // 8, generator=torch.Generator().manual_seed(11)).to(bf16)
     kw = dict(prompt="a corgi surfing", negative_prompt="blurry", video_length=FRAMES, height=H, width=W, num_inference_steps=2,
               guidance_scale=6.0, latents=lat)
-    want = ref(**kw).frames
     got = EasyAnimatePipeline(vae=v, transformer=t, tokenizer=tok, text_encoder=enc)(**kw).frames
-    _same(got, want)
-    e_ref = ref.encode_prompt("a corgi surfing", torch.device("cpu"), bf16, negative_prompt="blurry")
+    _same_ref("prompt_strings", got, lambda: ref(**kw).frames)
+    e_ref = ref.encode_prompt("a corgi surfing", torch.device("cpu"), bf16, negative_prompt="blurry") if LIVE else None
     e_ours = EasyAnimatePipeline(vae=v, transformer=t, tokenizer=tok, text_encoder=enc).encode_prompt(
         "a corgi surfing", torch.device("cpu"), bf16, negative_prompt="blurry")
-    assert all(torch.equal(a, b) for a, b in zip(e_ref, e_ours))
+    assert GOLD.value("prompt_embeds_count", _live(lambda: len(e_ref))) == len(e_ours)
+    for i, b in enumerate(e_ours):
+        GOLD.same_sample(f"prompt_embeds_{i}", b, e_ref[i] if LIVE else None)
 
 
 def test_teacache_inside_the_pipeline_call_matches_the_reference_pipeline(on_cpu):
@@ -260,12 +287,14 @@ def test_teacache_inside_the_pipeline_call_matches_the_reference_pipeline(on_cpu
     steps = 8
     kw = dict(video_length=FRAMES, height=H, width=W, num_inference_steps=steps, guidance_scale=6.0, latents=lat, **_mask_kw(pe, ne))
     t.enable_teacache(steps, 0.3, coefficients=coeffs)
-    want = ref_pipeline.reference_pipeline(t, v)(**kw).frames
-    skipped_ref = t.teacache.skipped
-    assert t.teacache.cnt == 0  # wrapped around after `steps` calls: ready for the next video
+    want = None
+    if LIVE:
+        want = ref_pipeline.reference_pipeline(t, v)(**kw).frames
+        assert t.teacache.cnt == 0  # wrapped around after `steps` calls: ready for the next video
+    skipped_ref = GOLD.value("teacache_skipped", _live(lambda: t.teacache.skipped))
     got = EasyAnimatePipeline(vae=v, transformer=t)(**kw).frames
-    assert 0 < skipped_ref < steps and t.teacache.skipped == 2 * skipped_ref
-    _same(got, want)
+    assert 0 < skipped_ref < steps and t.teacache.skipped == (2 if LIVE else 1) * skipped_ref and t.teacache.cnt == 0
+    _same_ref("teacache", got, lambda: want)
 
 
 def test_two_videos_per_prompt(on_cpu):
@@ -275,11 +304,10 @@ def test_two_videos_per_prompt(on_cpu):
     pe, ne = _embeds(torch.Generator().manual_seed(31))
     kw = dict(video_length=FRAMES, height=H, width=W, num_inference_steps=2, guidance_scale=6.0, num_images_per_prompt=2,
               **_mask_kw(pe, ne))
-    ref, pipe = ref_pipeline.reference_pipeline(t, v), EasyAnimatePipeline(vae=v, transformer=t)
-    want = ref(generator=torch.Generator().manual_seed(32), **kw).frames
+    pipe = EasyAnimatePipeline(vae=v, transformer=t)
     got = pipe(generator=torch.Generator().manual_seed(32), **kw).frames
     assert got.shape == (2, 3, FRAMES, H, W)
-    _same(got, want)
+    _same_ref("two_videos", got, lambda: ref_pipeline.reference_pipeline(t, v)(generator=torch.Generator().manual_seed(32), **kw).frames)
     with pytest.raises(ValueError, match="list of generators"):
         pipe(generator=[torch.Generator().manual_seed(1)] * 3, **kw)
 
@@ -332,10 +360,10 @@ def test_t2v_edge_shapes(on_cpu, video_length, h, w):
     t, v = _modules(on_cpu)
     pe, ne = _embeds(torch.Generator().manual_seed(41))
     kw = dict(video_length=video_length, height=h, width=w, num_inference_steps=2, guidance_scale=6.0, **_mask_kw(pe, ne))
-    want = ref_pipeline.reference_pipeline(t, v)(generator=torch.Generator().manual_seed(42), **kw).frames
     got = EasyAnimatePipeline(vae=v, transformer=t)(generator=torch.Generator().manual_seed(42), **kw).frames
     assert got.shape == (1, 3, video_length, h // 16 * 16, w // 16 * 16)
-    _same(got, want)
+    _same_ref(f"edge_{video_length}_{h}_{w}", got,
+              lambda: ref_pipeline.reference_pipeline(t, v)(generator=torch.Generator().manual_seed(42), **kw).frames)
 
 
 def test_inpaint_pipeline_with_vae_encoded_mask(on_cpu):
@@ -350,8 +378,8 @@ def test_inpaint_pipeline_with_vae_encoded_mask(on_cpu):
     pe, ne = _embeds(g)
     kw = dict(video_length=FRAMES, video=video, mask_video=mask, height=H, width=W, num_inference_steps=2, guidance_scale=6.0,
               **_mask_kw(pe, ne))
-    want = ref_pipeline.reference_inpaint_pipeline(t, v)(generator=torch.Generator().manual_seed(15), **kw).frames
-    _same(EasyAnimateInpaintPipeline(vae=v, transformer=t)(generator=torch.Generator().manual_seed(15), **kw).frames, want)
+    _same_ref("inpaint_vae_mask", EasyAnimateInpaintPipeline(vae=v, transformer=t)(generator=torch.Generator().manual_seed(15), **kw).frames,
+              lambda: ref_pipeline.reference_inpaint_pipeline(t, v)(generator=torch.Generator().manual_seed(15), **kw).frames)
 
 
 def test_inpaint_reference_video_noise_with_sampled_strength(on_cpu):
@@ -367,8 +395,10 @@ def test_inpaint_reference_video_noise_with_sampled_strength(on_cpu):
     pe, ne = _embeds(g)
     kw = dict(video_length=FRAMES, video=video, mask_video=mask, height=H, width=W, num_inference_steps=2, guidance_scale=6.0,
               noise_aug_strength=None, **_mask_kw(pe, ne))
-    torch.manual_seed(17)
-    want = ref_pipeline.reference_inpaint_pipeline(t, v)(generator=torch.Generator().manual_seed(18), **kw).frames
+    want = None
+    if LIVE:
+        torch.manual_seed(17)
+        want = ref_pipeline.reference_inpaint_pipeline(t, v)(generator=torch.Generator().manual_seed(18), **kw).frames
     torch.manual_seed(17)
     got = EasyAnimateInpaintPipeline(vae=v, transformer=t)(generator=torch.Generator().manual_seed(18), **kw).frames
-    _same(got, want)
+    _same_ref("inpaint_sampled_strength", got, lambda: want)

@@ -47,7 +47,7 @@ def test_vae_oracle_wrapper_matches_reference_golden():
     """decode / tiled_decode of the REFERENCE's AutoencoderKLMagvit wrapper (post_quant_conv, 3 x 3 tiles + the
     lower-right corner pass, blend_v / blend_h order): tests/golden/make_golden.py::make_vae_tiled."""
     path = os.path.join(GOLD, "vae_ref_tiled.safetensors")
-    t, meta = load_file(path), _meta(path)
+    t, meta = {**load_file(path), **load_file(os.path.join(GOLD, "vae_ref_tiled_2.safetensors"))}, _meta(path)
     boc = ast.literal_eval(meta["block_out_channels"])
     m = vae.init_weights_(vae.OracleAutoencoderKLMagvit(block_out_channels=boc, use_tiling=True,
                                                         tile_sample_min_size=int(meta["tile_sample_min_size"])), int(meta["seed"]))
@@ -74,7 +74,7 @@ def test_vae_oracle_wrapper_matches_live_reference():
 def test_vae_oracle_encode_matches_reference_golden():
     """encode / tiled_encode moments of the REFERENCE's AutoencoderKLMagvit (chunked Encoder: frame 0 alone, then four
     frames at a time with cached context): the whole-sequence encoder oracle reproduces them (I2V conditioning prep,
-    SURVEY.md section 8(f) 'next' row - no CUDA path yet)."""
+    no CUDA path yet)."""
     path = os.path.join(GOLD, "vae_ref_encode.safetensors")
     t, meta = load_file(path), _meta(path)
     boc = ast.literal_eval(meta["block_out_channels"])

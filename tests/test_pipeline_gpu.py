@@ -1,4 +1,4 @@
-"""Rows a1 / a10 / a17 of SURVEY.md section 8 on the GPU: the multi-step CFG sampler (pipeline_easyanimate.py:1065-1111) against
+"""On the GPU: the multi-step CFG sampler (pipeline_easyanimate.py:1065-1111) against
 the oracle's denoise loop, `decode_latents` (pipeline_easyanimate.py:722-742) including the fused scale / clamp / float32-to-host
 tail, and the checkpoint loaders (`from_pretrained_2d` with its `proj.weight` channel-resize shim, transformer3d.py:1775-1787;
 `AutoencoderKLMagvit.from_pretrained`, autoencoder_magvit.py:478-505).  Each test's GPU-free prelude also runs in the CPU
@@ -150,6 +150,7 @@ def prelude_reference_pipeline_golden(device="cuda"):
     reference's EasyAnimatePipeline.__call__ over the reference's transformer + VAE, in bf16 and in fp32.  The product modules
     load the same seeded, bf16-rounded weights."""
     from safetensors import safe_open
+    from safetensors.torch import load_file
     from easyanimate_b200.autoencoder_magvit import AutoencoderKLMagvit
     from easyanimate_b200.pipeline import EasyAnimateSampler
     from easyanimate_b200.transformer3d import EasyAnimateTransformer3DModel
@@ -158,6 +159,7 @@ def prelude_reference_pipeline_golden(device="cuda"):
     with safe_open(path, "pt") as f:
         t = {k: f.get_tensor(k) for k in f.keys()}
         meta = f.metadata()
+    t.update(load_file(path.replace(".safetensors", "_2.safetensors")))  # frames_fp32 (files are kept under 1 MB)
     ot, ov = G.pipeline_case_modules(bf16)
     lat, pe, ne = G.pipeline_case_inputs()
     assert torch.equal(lat, t["latents"]) and torch.equal(pe, t["prompt_embeds"]) and torch.equal(ne, t["negative_prompt_embeds"])

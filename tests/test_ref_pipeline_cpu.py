@@ -1,4 +1,4 @@
-"""SURVEY.md section 8b, the boundary's strongest proof available without a GPU: the REFERENCE's own
+"""The boundary's strongest proof available without a GPU: the REFERENCE's own
 `EasyAnimatePipeline.__call__` (easyanimate/pipeline/pipeline_easyanimate.py:769-1148, executed unmodified from
 /root/reference through oracle/ref_pipeline.py) driving
 

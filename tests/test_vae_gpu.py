@@ -31,10 +31,9 @@ def _ref_causal_conv(x_cl, w, b):
 
 @pytest.mark.parametrize("T,H,W,Cin,Cout", [(1, 8, 16, 64, 64), (3, 10, 20, 64, 128), (2, 9, 7, 128, 256), (4, 16, 32, 256, 128),
                                             (2, 24, 40, 512, 512),
-                                            # large enough for the 256-pixel CTA tiles (two sub-tiles per CTA), exact and ragged
+                                            # frames of many 128-pixel tiles, exact and ragged
                                             (5, 128, 160, 64, 128), (5, 122, 150, 64, 128), (3, 90, 160, 128, 256),
-                                            # large enough for CTA pairs (cta_group::2): 256-wide weight tile / 128-wide with
-                                            # two sub-tiles; odd number of tile rows so the last pair is half empty
+                                            # 256- and 128-wide weight tiles over more tiles than SMs (persistent tile loop)
                                             (3, 208, 256, 128, 256), (3, 400, 250, 64, 128)])
 def test_conv3d_causal(T, H, W, Cin, Cout):
     from easyanimate_b200 import vae_ops
@@ -58,7 +57,8 @@ def test_conv3d_causal(T, H, W, Cin, Cout):
 @pytest.mark.parametrize("variant", [0, 4])
 def test_conv3d_output_row_window_is_the_same_convolution(T, H, W, Cin, Cout, variant, monkeypatch):
     """ea_conv3d_args.out_row0 / out_rows (strip-parallel decode): the rows of a window are bit-identical to the same rows of the
-    whole-frame convolution, with residual, frame duplication and the planar store - both kernel families."""
+    whole-frame convolution, with residual, frame duplication and the planar store - for both accepted values of the ABI's
+    `variant` field (0 and the former tap-per-box bit 4, which now select the same kernel)."""
     from easyanimate_b200 import vae_ops
     monkeypatch.setattr(vae_ops, "CONV_VARIANT", variant)
     x = _rand((T, H, W, Cin), 1.0, 1)
@@ -247,7 +247,7 @@ def prelude_tiled_reference_golden():
     from oracle import vae
     from easyanimate_b200.autoencoder_magvit import AutoencoderKLMagvit
     path = os.path.join(GOLD, "vae_ref_tiled.safetensors")
-    t = load_file(path)
+    t = {**load_file(path), **load_file(os.path.join(GOLD, "vae_ref_tiled_2.safetensors"))}  # files are kept under 1 MB
     with safe_open(path, framework="pt") as f:
         meta = f.metadata()
     boc = list(ast.literal_eval(meta["block_out_channels"]))

@@ -1,4 +1,4 @@
-"""AutoencoderKLMagvit.encode on the GPU (I2V / inpaint conditioning prep, SURVEY.md section 8(f) rank 2).
+"""AutoencoderKLMagvit.encode on the GPU (I2V / inpaint conditioning prep).
 
 encode() runs the encoder's stride-2 convolutions as the strided implicit-GEMM kernel (ea_conv3d_causal with stride fields)
 or, for A/B, as the stride-1 kernel plus a strided pick; both are compared here with fp32 PyTorch references and with the
@@ -35,13 +35,12 @@ def test_strided_convolution_as_stride1_plus_pick():
 
 
 @pytest.mark.parametrize("T,H,W,Cin,Cout,st", [(5, 18, 22, 64, 64, 2), (5, 18, 22, 64, 64, 1), (9, 33, 47, 128, 128, 2), (1, 16, 16, 64, 128, 1),
-                                              # large enough for the 256-pixel CTA tiles and for CTA pairs
+                                              # frames of many 128-pixel tiles
                                               (5, 256, 320, 128, 128, 2), (3, 416, 512, 128, 256, 1)])
 def test_strided_convolution_kernel(T, H, W, Cin, Cout, st, monkeypatch):
     """ea_conv3d_causal with stride (st, 2, 2) (TMA element strides) against F.conv3d on the reference's padding recipe
-    (downsamplers.py:24-96), and bit for bit against the stride-1 form of the SAME kernel family (tap-per-box, variant bit 2)
-    + strided pick; the halo-tile kernel that unit-stride calls take by default walks k as (kt, channel slice, kh, kw)
-    instead of (tap, channel slice) and agrees to fp32 summation order."""
+    (downsamplers.py:24-96), and bit for bit against the stride-1 form of the same kernel + strided pick (with the ABI's
+    former tap-per-box variant bit set, which selects the same kernel)."""
     import torch.nn.functional as F
     from easyanimate_b200 import vae_ops
     g = torch.Generator(device="cuda").manual_seed(T * H + W)
@@ -55,13 +54,10 @@ def test_strided_convolution_kernel(T, H, W, Cin, Cout, st, monkeypatch):
     ref = F.conv3d(xin, w.float(), b.float(), stride=(st, 2, 2))[0].permute(1, 2, 3, 0)
     assert got.shape == ref.shape == ((T + 1) // 2 if st == 2 else T, H // 2, W // 2, Cout)
     torch.testing.assert_close(got.float(), ref, rtol=2 ** -7, atol=2e-2)
-    full_halo = vae_ops.conv3d_causal(x, wp, b, Cout)
     monkeypatch.setattr(vae_ops, "CONV_VARIANT", vae_ops.CONV_VARIANT | 4)
     full = vae_ops.conv3d_causal(x, wp, b, Cout)
     pick = (full[::2] if st == 2 else full)[:, 1::2, 1::2]
     assert torch.equal(got, pick[:, :H // 2, :W // 2])  # same taps, same k order, same accumulator: identical
-    pick_halo = (full_halo[::2] if st == 2 else full_halo)[:, 1::2, 1::2][:, :H // 2, :W // 2]
-    torch.testing.assert_close(got.float(), pick_halo.float(), rtol=2 ** -7, atol=2 ** -7)
 
 
 def prelude_encode_golden():

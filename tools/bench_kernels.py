@@ -73,7 +73,7 @@ def bench_attn():
 
 
 def vae_conv_flops(F_lat, h, w, boc=(128, 256, 512, 512), mid_attn=True):
-    """conv FLOPs of one untiled decode (BASELINE.md §2 / §4 tracer closed form for the released architecture)."""
+    """conv FLOPs of one untiled decode."""
     T1, T2, T3 = F_lat, 2 * F_lat - 1, 4 * F_lat - 3
     c0, c1, c2, c3 = boc  # 128,256,512,512
     def conv(T, H, W, cin, cout, k=27): return 2.0 * T * H * W * cout * cin * k

@@ -1,4 +1,4 @@
-"""Multi-GPU checks (run under torchrun on a B200 box, world 2 / 4 / 8):
+"""Multi-GPU checks (run under torchrun on a multi-GPU H100 machine, world 2 / 4 / 8):
   1. CFG-parallel sampler == single-GPU batch-of-2 sampler (world 2 only), bit for bit;
   2. sequence-parallel forward over ALL ranks == single-GPU forward, bit for bit, for both exchange implementations:
      the fused peer-store exchange (`p2p`: QKV-epilogue / attention-epilogue stores into CUDA-IPC-mapped peer buffers) and

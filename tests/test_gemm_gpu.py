@@ -77,36 +77,54 @@ def test_gemm_scale_f32_and_bias_res():
     _ulp_close(out2, ref2)
 
 
-@pytest.mark.parametrize("B,S_part,S,off,d,rope", [(2, 200, 264, 64, 256, True), (2, 64, 264, 0, 256, False),
-                                                   (1, 1000, 1256, 256, 3072, True)])
-def test_qkv_gemm_ln_rope(B, S_part, S, off, d, rope):
-    from easyanimate_b200 import ops
-    H = d // 64
-    a = _rand((B * S_part, d), 1.0, 1)
-    w, b = _rand((3 * d, d), 0.05, 2), _rand((3 * d,), 0.5, 3)
-    lnq = (1 + _rand((64,), 0.1, 4), _rand((64,), 0.1, 5))
-    lnk = (1 + _rand((64,), 0.1, 6), _rand((64,), 0.1, 7))
-    cos = sin = None
+def qkv_inputs(B, S_part, d, rope, seed=1):
+    """Random operands of ea_qkv_gemm_ln_rope: a [B*S_part, d], the fused weight / bias, the two LayerNorm affines and
+    (rope) interleaved cos / sin tables [S_part, 64]."""
+    a = _rand((B * S_part, d), 1.0, seed)
+    w, b = _rand((3 * d, d), 0.05, seed + 1), _rand((3 * d,), 0.5, seed + 2)
+    lnq = (1 + _rand((64,), 0.1, seed + 3), _rand((64,), 0.1, seed + 4))
+    lnk = (1 + _rand((64,), 0.1, seed + 5), _rand((64,), 0.1, seed + 6))
+    rope_cs = None
     if rope:
-        ang = torch.rand((S_part, 32), device="cuda") * 6.28
-        cos = torch.cos(ang).repeat_interleave(2, dim=1).contiguous()
-        sin = torch.sin(ang).repeat_interleave(2, dim=1).contiguous()
-    q = torch.zeros((B, H, S, 64), device="cuda", dtype=bf16)
-    k, v = torch.zeros_like(q), torch.zeros_like(q)
-    ops.qkv_gemm_ln_rope(a, w, b, lnq, lnk, (cos, sin) if rope else None, q, k, v, rows_per_batch=S_part,
-                         seq_offset=off, eps=1e-6)
-    lin = (a.float() @ w.float().t() + b.float()).to(bf16).view(B, S_part, 3, H, 64)
+        g = torch.Generator(device="cuda").manual_seed(seed + 7)
+        ang = torch.rand((S_part, 32), device="cuda", generator=g) * 6.28
+        rope_cs = (torch.cos(ang).repeat_interleave(2, dim=1).contiguous(),
+                   torch.sin(ang).repeat_interleave(2, dim=1).contiguous())
+    return a, w, b, lnq, lnk, rope_cs
+
+
+def qkv_reference(a, w, b, lnq, lnk, rope_cs, B, S_part):
+    """The projection + per-head LayerNorm + RoPE in torch: (q, k, v) [B, H, S_part, 64] bf16.  The GEMM is accumulated in
+    fp64 and rounded to fp32 before the bias, so v (no LayerNorm) is the kernel's bf16(acc + bias) up to accumulation order."""
+    d = a.shape[1]
+    H = d // 64
+    acc = (a.double() @ w.double().t()).float()
+    lin = (acc + b.float()).to(bf16).view(B, S_part, 3, H, 64)
     rq, rk, rv = [lin[:, :, i].transpose(1, 2) for i in range(3)]  # [B,H,S_part,64]
     rq = torch.nn.functional.layer_norm(rq, (64,), lnq[0], lnq[1], 1e-6)
     rk = torch.nn.functional.layer_norm(rk, (64,), lnk[0], lnk[1], 1e-6)
 
     def rot(x):
+        cos, sin = rope_cs
         xr, xi = x.reshape(*x.shape[:-1], -1, 2).unbind(-1)
         xrot = torch.stack([-xi, xr], dim=-1).flatten(3)
         return (x.float() * cos + xrot.float() * sin).to(x.dtype)
 
-    if rope:
+    if rope_cs is not None:
         rq, rk = rot(rq), rot(rk)
+    return rq, rk, rv
+
+
+@pytest.mark.parametrize("B,S_part,S,off,d,rope", [(2, 200, 264, 64, 256, True), (2, 64, 264, 0, 256, False),
+                                                   (1, 1000, 1256, 256, 3072, True)])
+def test_qkv_gemm_ln_rope(B, S_part, S, off, d, rope):
+    from easyanimate_b200 import ops
+    H = d // 64
+    a, w, b, lnq, lnk, rope_cs = qkv_inputs(B, S_part, d, rope)
+    q = torch.zeros((B, H, S, 64), device="cuda", dtype=bf16)
+    k, v = torch.zeros_like(q), torch.zeros_like(q)
+    ops.qkv_gemm_ln_rope(a, w, b, lnq, lnk, rope_cs, q, k, v, rows_per_batch=S_part, seq_offset=off, eps=1e-6)
+    rq, rk, rv = qkv_reference(a, w, b, lnq, lnk, rope_cs, B, S_part)
     for got, ref in ((q, rq), (k, rk), (v, rv)):
         _ulp_close(got[:, :, off:off + S_part], ref, rtol=2 ** -6, atol=3e-2)
         assert torch.count_nonzero(got[:, :, :off]) == 0 and torch.count_nonzero(got[:, :, off + S_part:]) == 0

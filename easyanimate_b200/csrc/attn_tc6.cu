@@ -269,16 +269,11 @@ static int launch(const ea_attn_args* g, cudaStream_t stream) {
       p.out_text_peers[i] = reinterpret_cast<bf16*>(pe->out_text[i]);
     }
   }
-  auto kern = attn6_kernel;
-  static ::ea::PerDeviceFlag attr_flag;
-  const int attr_dev = ::ea::current_device();
-  if (!attr_flag.get(attr_dev)) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kTotal);
-    if (e != cudaSuccess) return fail(EA_ERR_CUDA, std::string("cudaFuncSetAttribute(attn6): ") + cudaGetErrorString(e));
-    attr_flag.set(attr_dev);
-  }
+  static ::ea::PerDeviceFlag smem_done;
+  rc = set_max_dynamic_smem(reinterpret_cast<const void*>(attn6_kernel), kTotal, smem_done, "attn6_kernel");
+  if (rc) return rc;
   dim3 grid((unsigned)((g->S + kQT - 1) / kQT), (unsigned)BH);
-  kern<<<grid, kThreads, kTotal, stream>>>(tq, tk, tv, p);
+  attn6_kernel<<<grid, kThreads, kTotal, stream>>>(tq, tk, tv, p);
   count_launch();
   return check_launch("attn6_kernel");
 }

@@ -10,12 +10,19 @@ ARCH=(-gencode arch=compute_90a,code=sm_90a)
 FLAGS=("${ARCH[@]}" -O3 -std=c++17 -lineinfo -Xcompiler -fPIC --expt-relaxed-constexpr -Xptxas -v -I"$HERE/../../include")
 # objects of an earlier build for another architecture are rebuilt
 if [[ ! -f "$OBJ/.arch" || "$(cat "$OBJ/.arch")" != "${ARCH[*]}" ]]; then rm -f "$OBJ"/*.o; echo "${ARCH[*]}" > "$OBJ/.arch"; fi
+# an object is stale when it is older than its source or than any header a source can include
+headers=("$HERE"/*.cuh "$HERE"/*.h "$HERE/../../include/ea_b200.h")
+stale() {
+  local dep
+  for dep in "$@"; do [[ "$dep" -nt "$obj" ]] && return 0; done
+  return 1
+}
 pids=()
 objs=()
 for src in "$HERE"/*.cu; do
   obj="$OBJ/$(basename "${src%.cu}").o"
   objs+=("$obj")
-  if [[ ! -f "$obj" || "$src" -nt "$obj" || "$HERE/common.cuh" -nt "$obj" || "$HERE/host.h" -nt "$obj" || "$HERE/../../include/ea_b200.h" -nt "$obj" ]]; then
+  if [[ ! -f "$obj" ]] || stale "$src" "${headers[@]}"; then
     ( "$NVCC" "${FLAGS[@]}" -c "$src" -o "$obj" > "$obj.log" 2>&1 || { cat "$obj.log"; exit 1; } ) &
     pids+=($!)
   fi

@@ -30,6 +30,33 @@ EA_DEVICE float2 unpack_bf16x2(uint32_t u) {
   return __bfloat1622float2(v);
 }
 
+// x[j] += src[j] for j < N (N a multiple of 8; src 16-byte aligned, read through the read-only cache)
+template <int N>
+EA_DEVICE void add_bf16(float* x, const bf16* src) {
+  const uint4* p = reinterpret_cast<const uint4*>(src);
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+    uint4 b = __ldg(p + j);
+    float2 f0 = unpack_bf16x2(b.x), f1 = unpack_bf16x2(b.y), f2 = unpack_bf16x2(b.z), f3 = unpack_bf16x2(b.w);
+    x[j * 8 + 0] += f0.x; x[j * 8 + 1] += f0.y; x[j * 8 + 2] += f1.x; x[j * 8 + 3] += f1.y;
+    x[j * 8 + 4] += f2.x; x[j * 8 + 5] += f2.y; x[j * 8 + 6] += f3.x; x[j * 8 + 7] += f3.y;
+  }
+}
+
+// dst[j] = bf16(x[j]) for j < N (N a multiple of 8; dst 16-byte aligned), 16-byte stores
+template <int N>
+EA_DEVICE void store_bf16(bf16* dst, const float* x) {
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+    uint4 w;
+    w.x = pack_bf16x2(x[j * 8 + 0], x[j * 8 + 1]);
+    w.y = pack_bf16x2(x[j * 8 + 2], x[j * 8 + 3]);
+    w.z = pack_bf16x2(x[j * 8 + 4], x[j * 8 + 5]);
+    w.w = pack_bf16x2(x[j * 8 + 6], x[j * 8 + 7]);
+    reinterpret_cast<uint4*>(dst)[j] = w;
+  }
+}
+
 // A kernel that waits on an mbarrier which never completes would hang the GPU box; every wait is
 // bounded and traps (kills the context, surfaces as a CUDA error on the host) instead.
 #ifndef EA_MBAR_TIMEOUT_NS
@@ -43,7 +70,6 @@ EA_DEVICE void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
 }
 EA_DEVICE void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-EA_DEVICE void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 EA_DEVICE void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
@@ -94,14 +120,6 @@ EA_DEVICE void tma_load_2d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, 
       ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
-EA_DEVICE uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-EA_DEVICE void cluster_sync() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
 EA_DEVICE void tma_load_3d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2) {
   asm volatile(
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
@@ -113,14 +131,6 @@ EA_DEVICE void tma_load_4d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, 
       "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
       ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2),
       "r"(c3)
-      : "memory");
-}
-EA_DEVICE void tma_load_5d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2, int c3,
-                           int c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], "
-      "[%2];" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
       : "memory");
 }
 

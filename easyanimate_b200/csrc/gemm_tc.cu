@@ -1,26 +1,15 @@
 // Persistent, warp-specialised wgmma GEMM for sm_90a:  D[M,N] = epi(A[M,K] · W[N,K]^T).
 //
-//   warpgroup 0 (1 thread) : TMA producer — cp.async.bulk.tensor tiles of A (128x64) and W (BNx64) into a SWIZZLE_128B
-//                            shared-memory ring, completion on `full` mbarriers.
-//   warpgroups 1, 2        : consumers — rows [0,64) / [64,128) of the 128 x BN tile: wgmma.m64nBNk16 (bf16 -> fp32 in
-//                            registers) from both operands in shared memory, then the epilogue: the accumulators go through
-//                            a shared-memory staging buffer so that each thread owns one row of 32 (or 64) consecutive
-//                            columns, fused bias / GELU / gate+residual / per-head LayerNorm + RoPE, bf16 stores.
-// The producer keeps fetching the next tile's k-blocks while the consumers run the epilogue.
+// The TMA / wgmma pipeline is tc_pipeline.cuh: 128 x BN output tiles, one TMA box of A (128x64) and one of W (BNx64) per
+// k-block.  In the epilogue each thread owns one row of 32 (or, for QKV, 64) consecutive staged columns: fused bias /
+// GELU / gate+residual / per-head LayerNorm + RoPE, bf16 stores.
 //
 // Replaces the cuBLAS calls behind every nn.Linear of the reference path (see include/ea_b200.h for call sites).
-#include "common.cuh"
 #include "host.h"
+#include "tc_pipeline.cuh"
 #include "../../include/ea_b200.h"
 
 namespace ea {
-
-extern void count_launch();
-
-constexpr int kBM = 128;
-constexpr int kBK = 64;
-constexpr int kGemmThreads = 384;
-constexpr int kStagePitch = 132;  // fp32 staging row pitch: conflict-free 16-byte row reads
 
 enum { EPI_QKV = 100 };
 
@@ -58,28 +47,16 @@ struct GemmDevArgs {
   bf16* v_peers[EA_MAX_PEERS];
 };
 
-template <int BN>
-struct GemmCfg {
-  static constexpr int kStages = BN == 256 ? 3 : (BN == 128 ? 4 : 6);
-  static constexpr int kABytes = kBM * kBK * 2;
-  static constexpr int kBBytes = BN * kBK * 2;
-  static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kCW = BN < 128 ? BN : 128;  // columns staged per epilogue pass
-  static constexpr int kStagingBytes = 2 * 64 * kStagePitch * 4;
-  static constexpr int kSmemBytes = kStages * kStageBytes + kStagingBytes + 1024 /*align slack*/ + 256 /*barriers*/;
-  static_assert(kSmemBytes <= 227 * 1024, "shared memory");
-};
-
 // ------------------------------------------------------------------------------------------------
-// epilogue helpers: one thread owns one accumulator row, `v` holds 32 consecutive columns
+// epilogue helpers: one thread owns one accumulator row, `x` holds 32 consecutive columns
 // ------------------------------------------------------------------------------------------------
 // Ragged right edge (N % 32 != 0): same arithmetic as the vector path, one column at a time.
 template <int EPI>
-EA_DEVICE void epilogue_tail(const GemmDevArgs& p, int row, int col0, int nvalid, uint32_t (&acc)[32]) {
+EA_DEVICE void epilogue_tail(const GemmDevArgs& p, int row, int col0, int nvalid, const float (&x)[32]) {
 #pragma unroll 1
   for (int j = 0; j < nvalid; ++j) {
     const int col = col0 + j;
-    float v = __uint_as_float(acc[j]);
+    float v = x[j];
     if constexpr (EPI == EA_EPI_SCALE_F32) {
       reinterpret_cast<float*>(p.out)[(int64_t)row * p.ldo + col] = v * p.scale;
     } else {
@@ -98,7 +75,7 @@ EA_DEVICE void epilogue_tail(const GemmDevArgs& p, int row, int col0, int nvalid
 }
 
 template <int EPI>
-EA_DEVICE void epilogue_chunk32(const GemmDevArgs& p, int row, int col0, uint32_t (&acc)[32]) {
+EA_DEVICE void epilogue_chunk32(const GemmDevArgs& p, int row, int col0, const float (&acc)[32]) {
   // row < M guaranteed by caller
   if (col0 + 32 > p.N) {
     epilogue_tail<EPI>(p, row, col0, p.N - col0, acc);
@@ -107,29 +84,14 @@ EA_DEVICE void epilogue_chunk32(const GemmDevArgs& p, int row, int col0, uint32_
   if constexpr (EPI == EA_EPI_SCALE_F32) {
     float* o = reinterpret_cast<float*>(p.out) + (int64_t)row * p.ldo + col0;
 #pragma unroll
-    for (int j = 0; j < 32; j += 4) {
-      float4 f;
-      f.x = __uint_as_float(acc[j]) * p.scale;
-      f.y = __uint_as_float(acc[j + 1]) * p.scale;
-      f.z = __uint_as_float(acc[j + 2]) * p.scale;
-      f.w = __uint_as_float(acc[j + 3]) * p.scale;
-      *reinterpret_cast<float4*>(o + j) = f;
-    }
-    return;
+    for (int j = 0; j < 32; j += 4)
+      *reinterpret_cast<float4*>(o + j) =
+          make_float4(acc[j] * p.scale, acc[j + 1] * p.scale, acc[j + 2] * p.scale, acc[j + 3] * p.scale);
   } else {
     float x[32];
 #pragma unroll
-    for (int j = 0; j < 32; ++j) x[j] = __uint_as_float(acc[j]);
-    if (p.bias != nullptr) {
-      const uint4* bp = reinterpret_cast<const uint4*>(p.bias + col0);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        uint4 b = __ldg(bp + j);
-        float2 f0 = unpack_bf16x2(b.x), f1 = unpack_bf16x2(b.y), f2 = unpack_bf16x2(b.z), f3 = unpack_bf16x2(b.w);
-        x[j * 8 + 0] += f0.x; x[j * 8 + 1] += f0.y; x[j * 8 + 2] += f1.x; x[j * 8 + 3] += f1.y;
-        x[j * 8 + 4] += f2.x; x[j * 8 + 5] += f2.y; x[j * 8 + 6] += f3.x; x[j * 8 + 7] += f3.y;
-      }
-    }
+    for (int j = 0; j < 32; ++j) x[j] = acc[j];
+    if (p.bias != nullptr) add_bf16<32>(x, p.bias + col0);
     // the reference materialises the Linear output in bf16 before the next op
 #pragma unroll
     for (int j = 0; j < 32; ++j) x[j] = bf16_round(x[j]);
@@ -159,30 +121,8 @@ EA_DEVICE void epilogue_chunk32(const GemmDevArgs& p, int row, int col0, uint32_
         }
       }
     }
-    if constexpr (EPI == EA_EPI_BIAS_RES) {
-      const uint4* rp = reinterpret_cast<const uint4*>(p.residual + (int64_t)row * p.ldr + col0);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        uint4 r = __ldg(rp + j);
-        uint32_t rw[4] = {r.x, r.y, r.z, r.w};
-#pragma unroll
-        for (int t = 0; t < 4; ++t) {
-          float2 rf = unpack_bf16x2(rw[t]);
-          x[j * 8 + 2 * t] += rf.x;
-          x[j * 8 + 2 * t + 1] += rf.y;
-        }
-      }
-    }
-    bf16* o = reinterpret_cast<bf16*>(p.out) + (int64_t)row * p.ldo + col0;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      uint4 w;
-      w.x = pack_bf16x2(x[j * 8 + 0], x[j * 8 + 1]);
-      w.y = pack_bf16x2(x[j * 8 + 2], x[j * 8 + 3]);
-      w.z = pack_bf16x2(x[j * 8 + 4], x[j * 8 + 5]);
-      w.w = pack_bf16x2(x[j * 8 + 6], x[j * 8 + 7]);
-      *reinterpret_cast<uint4*>(o + j * 8) = w;
-    }
+    if constexpr (EPI == EA_EPI_BIAS_RES) add_bf16<32>(x, p.residual + (int64_t)row * p.ldr + col0);
+    store_bf16<32>(reinterpret_cast<bf16*>(p.out) + (int64_t)row * p.ldo + col0, x);
   }
 }
 
@@ -191,16 +131,7 @@ EA_DEVICE void epilogue_qkv_head(const GemmDevArgs& p, int row, int col0, const 
   float x[64];
 #pragma unroll
   for (int j = 0; j < 64; j += 4) *reinterpret_cast<float4*>(x + j) = *reinterpret_cast<const float4*>(src + j);
-  {
-    const uint4* bp = reinterpret_cast<const uint4*>(p.bias + col0);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      uint4 b = __ldg(bp + j);
-      float2 f0 = unpack_bf16x2(b.x), f1 = unpack_bf16x2(b.y), f2 = unpack_bf16x2(b.z), f3 = unpack_bf16x2(b.w);
-      x[j * 8 + 0] += f0.x; x[j * 8 + 1] += f0.y; x[j * 8 + 2] += f1.x; x[j * 8 + 3] += f1.y;
-      x[j * 8 + 4] += f2.x; x[j * 8 + 5] += f2.y; x[j * 8 + 6] += f3.x; x[j * 8 + 7] += f3.y;
-    }
-  }
+  add_bf16<64>(x, p.bias + col0);
 #pragma unroll
   for (int j = 0; j < 64; ++j) x[j] = bf16_round(x[j]);
 
@@ -270,138 +201,38 @@ EA_DEVICE void epilogue_qkv_head(const GemmDevArgs& p, int row, int col0, const 
     head_l = head - owner * p.heads_per_peer;
     heads_l = p.heads_per_peer;
   }
-  bf16* o = base + (((int64_t)b * heads_l + head_l) * p.S + p.seq_offset + s) * 64;
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    uint4 w;
-    w.x = pack_bf16x2(x[j * 8 + 0], x[j * 8 + 1]);
-    w.y = pack_bf16x2(x[j * 8 + 2], x[j * 8 + 3]);
-    w.z = pack_bf16x2(x[j * 8 + 4], x[j * 8 + 5]);
-    w.w = pack_bf16x2(x[j * 8 + 6], x[j * 8 + 7]);
-    *reinterpret_cast<uint4*>(o + j * 8) = w;
-  }
+  store_bf16<64>(base + (((int64_t)b * heads_l + head_l) * p.S + p.seq_offset + s) * 64, x);
 }
 
 // ------------------------------------------------------------------------------------------------
 // kernel
 // ------------------------------------------------------------------------------------------------
 template <int BN, int EPI>
-__global__ void __launch_bounds__(kGemmThreads, 1)
+__global__ void __launch_bounds__(kTcThreads, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                const GemmDevArgs p) {
-  using Cfg = GemmCfg<BN>;
-  constexpr int kStages = Cfg::kStages;
-  constexpr int kCW = Cfg::kCW;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + kStages * Cfg::kABytes;
-  float* staging = reinterpret_cast<float*>(smem + kStages * Cfg::kStageBytes);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * Cfg::kStageBytes + Cfg::kStagingBytes);
-  uint64_t* full_bar = bars;
-  uint64_t* empty_bar = bars + kStages;
-
-  const int wg = threadIdx.x >> 7;
-  const int lane = threadIdx.x & 31;
-
-  const int num_m_tiles = (p.M + kBM - 1) / kBM;
   const int num_n_tiles = (p.N + BN - 1) / BN;
-  const int num_tiles = num_m_tiles * num_n_tiles;
-  const int num_k_blocks = (p.K + kBK - 1) / kBK;
-
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmap_a);
-    tma_prefetch_desc(&tmap_b);
-    for (int i = 0; i < kStages; ++i) {
-      mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 8);  // lane 0 of each consumer warp
-    }
-    fence_mbar_init();
-  }
-  __syncthreads();
-
-  if (wg == 0) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
-    if (threadIdx.x == 0) {
-      // ===== TMA producer =====
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int m0 = (tile / num_n_tiles) * kBM;
-        const int n0 = (tile % num_n_tiles) * BN;
-        for (int kb = 0; kb < num_k_blocks; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          mbar_arrive_expect_tx(&full_bar[stage], Cfg::kStageBytes);
-          tma_load_2d(smem_a + stage * Cfg::kABytes, &tmap_a, &full_bar[stage], kb * kBK, m0);
-          tma_load_2d(smem_b + stage * Cfg::kBBytes, &tmap_b, &full_bar[stage], kb * kBK, n0);
-          if (++stage == kStages) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
-    // ===== consumers: rows [64 (wg-1), 64 wg) of the tile =====
-    const int cw = wg - 1;
-    const int tid = threadIdx.x & 127;
-    float* stage_buf = staging + cw * 64 * kStagePitch;
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int m0 = (tile / num_n_tiles) * kBM;
-      const int n0 = (tile % num_n_tiles) * BN;
-      float acc[BN / 2];
-      int prev = -1;
-      for (int kb = 0; kb < num_k_blocks; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        const uint64_t adesc = gmma_desc_sw128(smem_u32(smem_a + stage * Cfg::kABytes + cw * 64 * 128));
-        const uint64_t bdesc = gmma_desc_sw128(smem_u32(smem_b + stage * Cfg::kBBytes));
-        wgmma_fence();
+  const int num_tiles = ((p.M + kTcBM - 1) / kTcBM) * num_n_tiles;
+  // tile -> (m0, n0): its first row of A and of W
+  auto decode = [&](int tile) { return make_int2((tile / num_n_tiles) * kTcBM, (tile % num_n_tiles) * BN); };
+  auto load = [](int2 mn, int kb, const CUtensorMap* ta, const CUtensorMap* tb, void* a, void* b, uint64_t* bar) {
+    tma_load_2d(a, ta, bar, kb * kTcBK, mn.x);
+    tma_load_2d(b, tb, bar, kb * kTcBK, mn.y);
+  };
+  // one row of 32 columns, or for QKV of one head (64 columns), per item
+  auto epilogue = [&](int2 mn, int r, int c, const float* src) {
+    const int row = mn.x + r, col = mn.y + c;
+    if (row >= p.M || col >= p.N) return;
+    if constexpr (EPI == EPI_QKV) {
+      epilogue_qkv_head(p, row, col, src);
+    } else {
+      float x[32];
 #pragma unroll
-        for (int k = 0; k < kBK / 16; ++k) {
-          // advance 16 bf16 = 32 B inside the 128 B swizzle row: +2 in the (addr >> 4) field
-          wgmma_ss<BN>(acc, adesc + 2 * k, bdesc + 2 * k, (kb | k) != 0);
-        }
-        wgmma_commit();
-        wgmma_wait<1>();  // the k-block before this one has been read: release its stage
-        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
-        prev = stage;
-        if (++stage == kStages) { stage = 0; phase ^= 1; }
-      }
-      wgmma_wait<0>();
-      reg_fence<BN / 2>(acc);
-      if (lane == 0) mbar_arrive(&empty_bar[prev]);
-
-      // ===== epilogue: kCW columns at a time through the staging buffer, one row per thread and column chunk =====
-#pragma unroll
-      for (int cb = 0; cb < BN / kCW; ++cb) {
-        named_bar_sync(1 + cw, 128);  // the previous pass has finished reading the staging buffer
-        stage_acc<kCW>(acc + cb * (kCW / 2), stage_buf, kStagePitch);
-        named_bar_sync(1 + cw, 128);
-        const int c0 = n0 + cb * kCW;
-        if constexpr (EPI == EPI_QKV) {
-#pragma unroll 1
-          for (int i = tid; i < 64 * (kCW / 64); i += 128) {
-            const int r = i & 63, h = i >> 6;
-            const int row = m0 + cw * 64 + r;
-            if (row < p.M && c0 + h * 64 < p.N) epilogue_qkv_head(p, row, c0 + h * 64, stage_buf + r * kStagePitch + h * 64);
-          }
-        } else {
-#pragma unroll 1
-          for (int i = tid; i < 64 * (kCW / 32); i += 128) {
-            const int r = i & 63, c = i >> 6;
-            const int row = m0 + cw * 64 + r;
-            if (row < p.M && c0 + c * 32 < p.N) {
-              uint32_t a32[32];
-              const float* src = stage_buf + r * kStagePitch + c * 32;
-#pragma unroll
-              for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4*>(a32 + j) = *reinterpret_cast<const float4*>(src + j);
-              epilogue_chunk32<EPI>(p, row, c0 + c * 32, a32);
-            }
-          }
-        }
-      }
+      for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4*>(x + j) = *reinterpret_cast<const float4*>(src + j);
+      epilogue_chunk32<EPI>(p, row, col, x);
     }
-  }
+  };
+  tc_pipeline<BN, EPI == EPI_QKV ? 64 : 32>(&tmap_a, &tmap_b, num_tiles, (p.K + kTcBK - 1) / kTcBK, decode, load, epilogue);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -410,35 +241,25 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
 template <int BN, int EPI>
 static int launch_gemm(const void* a, int64_t lda, const void* w, int64_t ldw, const GemmDevArgs& p,
                        cudaStream_t stream) {
-  using Cfg = GemmCfg<BN>;
   CUtensorMap ta, tb;
   {
     uint64_t dims[2] = {(uint64_t)p.K, (uint64_t)p.M};
     uint64_t strides[1] = {(uint64_t)lda * 2};
-    uint32_t box[2] = {kBK, kBM};
+    uint32_t box[2] = {kTcBK, kTcBM};
     int rc = make_tmap_bf16(&ta, a, 2, dims, strides, box, true);
     if (rc) return rc;
   }
   {
     uint64_t dims[2] = {(uint64_t)p.K, (uint64_t)p.N};
     uint64_t strides[1] = {(uint64_t)ldw * 2};
-    uint32_t box[2] = {kBK, (uint32_t)BN};
+    uint32_t box[2] = {kTcBK, (uint32_t)BN};
     int rc = make_tmap_bf16(&tb, w, 2, dims, strides, box, true);
     if (rc) return rc;
   }
-  auto kern = gemm_tc_kernel<BN, EPI>;
-  static ::ea::PerDeviceFlag attr_flag;
-  const int attr_dev = ::ea::current_device();
-  if (!attr_flag.get(attr_dev)) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
-    if (e != cudaSuccess) return fail(EA_ERR_CUDA, std::string("cudaFuncSetAttribute(gemm): ") + cudaGetErrorString(e));
-    attr_flag.set(attr_dev);
-  }
-  const int num_tiles = ((p.M + kBM - 1) / kBM) * ((p.N + BN - 1) / BN);
-  int grid = num_tiles < sm_count() ? num_tiles : sm_count();
-  kern<<<grid, kGemmThreads, Cfg::kSmemBytes, stream>>>(ta, tb, p);
-  count_launch();
-  return check_launch("gemm_tc_kernel");
+  static PerDeviceFlag smem_done;
+  const int num_tiles = ((p.M + kTcBM - 1) / kTcBM) * ((p.N + BN - 1) / BN);
+  return launch_persistent(gemm_tc_kernel<BN, EPI>, num_tiles, kTcThreads, TcCfg<BN>::kSmemBytes, smem_done, stream,
+                           "gemm_tc_kernel", ta, tb, p);
 }
 
 template <int EPI>
@@ -446,7 +267,7 @@ static int dispatch_bn(const void* a, int64_t lda, const void* w, int64_t ldw, c
                        cudaStream_t stream) {
   // Wide tiles unless they would leave most SMs idle.
   const int sms = sm_count();
-  auto tiles = [&](int bn) { return (int64_t)((p.M + kBM - 1) / kBM) * ((p.N + bn - 1) / bn); };
+  auto tiles = [&](int bn) { return (int64_t)((p.M + kTcBM - 1) / kTcBM) * ((p.N + bn - 1) / bn); };
   // (ragged N is fine for every width: TMA zero-fills the missing weight rows, the epilogue masks the columns)
   if (p.N >= 256 && tiles(256) >= sms) return launch_gemm<256, EPI>(a, lda, w, ldw, p, stream);
   if (p.N >= 128 && tiles(128) >= sms / 2) return launch_gemm<128, EPI>(a, lda, w, ldw, p, stream);

@@ -6,7 +6,6 @@ namespace ea {
 
 static thread_local std::string g_last_error;
 
-void set_error(const std::string& msg) { g_last_error = msg; }
 int fail(int code, const std::string& msg) {
   g_last_error = msg;
   return code;
@@ -80,6 +79,15 @@ int sm_count() {
     n[dev] = v > 0 ? v : 132;
   }
   return n[dev];
+}
+
+int set_max_dynamic_smem(const void* kern, int bytes, PerDeviceFlag& done, const char* what) {
+  const int dev = current_device();
+  if (done.get(dev)) return EA_OK;
+  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  if (e != cudaSuccess) return fail(EA_ERR_CUDA, std::string("cudaFuncSetAttribute(") + what + "): " + cudaGetErrorString(e));
+  done.set(dev);
+  return EA_OK;
 }
 
 }  // namespace ea

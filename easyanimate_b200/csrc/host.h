@@ -1,4 +1,4 @@
-// Host-side helpers shared by the C-ABI translation units: error reporting, TMA descriptor encoding
+// Host-side helpers shared by the C-ABI translation units: error reporting, kernel launch, TMA descriptor encoding
 // (cuTensorMapEncodeTiled looked up through the runtime so the library has no link-time libcuda dependency).
 #pragma once
 #include <cuda.h>
@@ -11,8 +11,6 @@
 
 namespace ea {
 
-
-void set_error(const std::string& msg);
 int fail(int code, const std::string& msg);
 int check_launch(const char* what);
 
@@ -35,6 +33,24 @@ struct PerDeviceFlag {
     if (dev >= 0 && dev < 64) done[dev] = true;
   }
 };
+
+void count_launch();
+
+// Raises kern's dynamic shared-memory limit to `bytes` on the current device, once per device (`done` belongs to kern).
+int set_max_dynamic_smem(const void* kern, int bytes, PerDeviceFlag& done, const char* what);
+
+// Launches kern(args...) as a persistent grid of min(tiles, SMs) CTAs of `threads` with `smem_bytes` of dynamic shared
+// memory (set_max_dynamic_smem with `smem_done` first), counts the launch and reports a launch error.
+template <class... Args>
+int launch_persistent(void (*kern)(Args...), int64_t tiles, int threads, int smem_bytes, PerDeviceFlag& smem_done,
+                      cudaStream_t stream, const char* what, const Args&... args) {
+  const int rc = set_max_dynamic_smem(reinterpret_cast<const void*>(kern), smem_bytes, smem_done, what);
+  if (rc) return rc;
+  const int grid = (int)(tiles < sm_count() ? tiles : sm_count());
+  kern<<<grid, threads, smem_bytes, stream>>>(args...);
+  count_launch();
+  return check_launch(what);
+}
 
 }  // namespace ea
 

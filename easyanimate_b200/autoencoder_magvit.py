@@ -58,6 +58,26 @@ class _PackedConv(nn.Conv3d):
         return vae_ops.conv3d_causal(x, self.packed(), self.bias, self.out_channels, **kw)
 
 
+class _WholeFrame:
+    """The four primitives the layer sequence below is written against, for whole frames on one GPU.  vae_strips.StripDecoder
+    supplies the same four for one horizontal strip of the frame; every `run(x, ex)` takes either."""
+
+    def conv(self, c: _PackedConv, x, **kw):
+        return c.run(x, **kw)
+
+    def gn(self, norm: nn.GroupNorm, x, silu):
+        return vae_ops.groupnorm(x, norm.weight, norm.bias, norm.num_groups, norm.eps, silu)
+
+    def attn(self, a: "_SpatialAttention", n, x):
+        return a.attend(n, x)
+
+    def upsample(self, x):
+        return vae_ops.upsample2x(x)
+
+
+_WHOLE_FRAME = _WholeFrame()
+
+
 class _ResBlock(nn.Module):  # common.py:254-323
     def __init__(self, cin, cout, groups, eps=1e-6):
         super().__init__()
@@ -67,17 +87,17 @@ class _ResBlock(nn.Module):  # common.py:254-323
         self.conv2 = _PackedConv(cout, cout)
         self.shortcut = nn.Conv3d(cin, cout, kernel_size=1) if cin != cout else nn.Identity()
 
-    def run(self, x):
+    def run(self, x, ex):
         T, H, W, Cin = x.shape
         if isinstance(self.shortcut, nn.Identity):
             sc = x
         else:
             co = self.shortcut.out_channels
             sc = ops.gemm(x.view(T * H * W, Cin), self.shortcut.weight.view(co, Cin), self.shortcut.bias).view(T, H, W, co)
-        h = vae_ops.groupnorm(x, self.norm1.weight, self.norm1.bias, self.norm1.num_groups, self.norm1.eps, True)
-        h = self.conv1.run(h)
-        h = vae_ops.groupnorm(h, self.norm2.weight, self.norm2.bias, self.norm2.num_groups, self.norm2.eps, True)
-        return self.conv2.run(h, residual=sc)
+        h = ex.gn(self.norm1, x, True)
+        h = ex.conv(self.conv1, h)
+        h = ex.gn(self.norm2, h, True)
+        return ex.conv(self.conv2, h, residual=sc)
 
 
 class _SpatialAttention(nn.Module):  # vaemodules/attention.py:63-160,391-423
@@ -99,14 +119,18 @@ class _SpatialAttention(nn.Module):  # vaemodules/attention.py:63-160,391-423
                            torch.cat([p.detach() for p in ps[3:]], 0).contiguous())
         return self._fused[1], self._fused[2]
 
-    def run(self, x):
-        T, H, W, Cc = x.shape
-        gn = self.group_norm
-        n = vae_ops.groupnorm(x, gn.weight, gn.bias, gn.num_groups, gn.eps, False)
+    def run(self, x, ex):
+        return ex.attn(self, ex.gn(self.group_norm, x, False), x)
+
+    def attend(self, n, x, **kw):
+        """n [T,H,W,C]: the normalised whole frames (keys / values); x [T,Hq,W,C]: the residual, one row per query (all of
+        the frame, or with q_rows=(first, last) the pixels of n that a strip owns)."""
+        T, H, W, Cc = n.shape
+        Hq = x.shape[1]
         w, b = self._qkv()
         out = vae_ops.spatial_attention(n.view(T * H * W, Cc), w, b, self.to_out.weight, self.to_out.bias,
-                                        x.view(T * H * W, Cc), T, self.scale)
-        return out.view(T, H, W, Cc)
+                                        x.view(T * Hq * W, Cc), T, self.scale, **kw)
+        return out.view(T, Hq, W, Cc)
 
 
 class _MidBlock(nn.Module):  # mid_blocks.py:38-196
@@ -118,12 +142,12 @@ class _MidBlock(nn.Module):  # mid_blocks.py:38-196
             self.attentions.append(_SpatialAttention(channels, groups) if add_attention else None)
             self.convs.append(_ResBlock(channels, channels, groups))
 
-    def run(self, x):
-        x = self.convs[0].run(x)
+    def run(self, x, ex):
+        x = self.convs[0].run(x, ex)
         for attn, res in zip(self.attentions, self.convs[1:]):
             if attn is not None:
-                x = attn.run(x)
-            x = res.run(x)
+                x = attn.run(x, ex)
+            x = res.run(x, ex)
         return x
 
 
@@ -133,10 +157,10 @@ class _Upsampler(nn.Module):  # upsamplers.py:21-37,123-153
         self.conv = _PackedConv(channels, channels)
         self.temporal = temporal
 
-    def run(self, x):
-        x = vae_ops.upsample2x(x)
+    def run(self, x, ex):
+        x = ex.upsample(x)
         # nearest temporal x2 of every frame but the first is fused into the conv's store
-        return self.conv.run(x, dup_frames=self.temporal and x.shape[0] > 1)
+        return ex.conv(self.conv, x, dup_frames=self.temporal and x.shape[0] > 1)
 
 
 class _UpBlock(nn.Module):  # up_blocks.py:96-147,344-395
@@ -145,11 +169,11 @@ class _UpBlock(nn.Module):  # up_blocks.py:96-147,344-395
         self.convs = nn.ModuleList([_ResBlock(cin if i == 0 else cout, cout, groups) for i in range(num_layers)])
         self.upsampler = _Upsampler(cin if upsampler_on_input else cout, temporal) if add_upsample else None
 
-    def run(self, x):
+    def run(self, x, ex):
         for c in self.convs:
-            x = c.run(x)
+            x = c.run(x, ex)
         if self.upsampler is not None:
-            x = self.upsampler.run(x)
+            x = self.upsampler.run(x, ex)
         return x
 
 
@@ -175,15 +199,15 @@ class _Decoder(nn.Module):  # omnigen_enc_dec.py:339-677
         self.conv_norm_out = nn.GroupNorm(norm_num_groups, block_out_channels[0], eps=1e-6)
         self.conv_out = _PackedConv(block_out_channels[0], out_channels, cout_pad=32)
 
-    def run(self, x):
-        """x [T,h,w,64] channels-last (post_quant_conv already applied) -> planar [3,T',8h,8w]."""
-        x = self.conv_in.run(x)
-        x = self.mid_block.run(x)
+    def run(self, x, ex):
+        """x [T,h,w,64] channels-last (post_quant_conv already applied) -> planar [3,T',8h,8w]; with a strip executor, the
+        strip's rows of both."""
+        x = ex.conv(self.conv_in, x)
+        x = self.mid_block.run(x, ex)
         for up in self.up_blocks:
-            x = up.run(x)
-        n = self.conv_norm_out
-        x = vae_ops.groupnorm(x, n.weight, n.bias, n.num_groups, n.eps, True)
-        return self.conv_out.run(x, out_planar=True)
+            x = up.run(x, ex)
+        x = ex.gn(self.conv_norm_out, x, True)
+        return ex.conv(self.conv_out, x, out_planar=True)
 
 
 class _Downsampler(nn.Module):  # downsamplers.py:24-46 (spatial), :74-96 (spatial + temporal)
@@ -194,14 +218,14 @@ class _Downsampler(nn.Module):  # downsamplers.py:24-46 (spatial), :74-96 (spati
 
     strided_kernel = os.environ.get("EA_ENC_STRIDED", "1") != "0"  # 0: stride-1 kernel + strided pick (A/B, 4-8x the FLOPs)
 
-    def run(self, x):
+    def run(self, x, ex):
         # CausalConv3d(kernel 3, stride (s_t, 2, 2), no spatial padding) after F.pad(x, (0,1,0,1)): output (t,i,j) reads
         # frames 2t-2..2t (clamped at 0) and pixels 2i..2i+2 / 2j..2j+2 with zeros past the right/bottom edge.  The
         # implicit-GEMM kernel does that directly (TMA element strides, ea_conv3d_args.stride_*); it is also output
         # (s_t*t, 2i+1, 2j+1) of the stride-1 causal convolution with 1-pixel zero padding, which the A/B path picks from.
         if self.strided_kernel:
-            return self.conv.run(x, stride_t=2 if self.temporal else 1, stride_hw=2)
-        y = self.conv.run(x)
+            return ex.conv(self.conv, x, stride_t=2 if self.temporal else 1, stride_hw=2)
+        y = ex.conv(self.conv, x)
         if self.temporal:
             y = y[::2]
         return y[:, 1::2, 1::2].contiguous()
@@ -213,11 +237,11 @@ class _DownBlock(nn.Module):  # down_blocks.py:156-212, 272-328
         self.convs = nn.ModuleList([_ResBlock(cin if i == 0 else cout, cout, groups) for i in range(num_layers)])
         self.downsampler = _Downsampler(cout, temporal) if add_downsample else None
 
-    def run(self, x):
+    def run(self, x, ex):
         for c in self.convs:
-            x = c.run(x)
+            x = c.run(x, ex)
         if self.downsampler is not None:
-            x = self.downsampler.run(x)
+            x = self.downsampler.run(x, ex)
         return x
 
 
@@ -239,15 +263,14 @@ class _Encoder(nn.Module):  # omnigen_enc_dec.py:24-337
         self.conv_norm_out = nn.GroupNorm(norm_num_groups, block_out_channels[-1], eps=1e-6)
         self.conv_out = _PackedConv(block_out_channels[-1], 2 * latent_channels, cout_pad=32)
 
-    def run(self, x):
+    def run(self, x, ex):
         """x [T,H,W,64] channels-last (RGB in the first 3 channels) -> planar [2*latent, T', H/8, W/8]."""
-        x = self.conv_in.run(x)
+        x = ex.conv(self.conv_in, x)
         for down in self.down_blocks:
-            x = down.run(x)
-        x = self.mid_block.run(x)
-        n = self.conv_norm_out
-        x = vae_ops.groupnorm(x, n.weight, n.bias, n.num_groups, n.eps, True)
-        return self.conv_out.run(x, out_planar=True)
+            x = down.run(x, ex)
+        x = self.mid_block.run(x, ex)
+        x = ex.gn(self.conv_norm_out, x, True)
+        return ex.conv(self.conv_out, x, out_planar=True)
 
 
 def _require_cuda(t: torch.Tensor, what: str) -> None:
@@ -255,6 +278,28 @@ def _require_cuda(t: torch.Tensor, what: str) -> None:
     the kernels for torch stand-ins, can lift exactly this guard and nothing else.)"""
     if not t.is_cuda:
         raise L.EaError(f"easyanimate_b200 has no CPU path: {what} must be on a CUDA device")
+
+
+def _stitch_tiles(rows, blend_extent: int, row_limit: int) -> torch.Tensor:
+    """rows[i][j] [1,C,T,h,w]: overlapping tiles in row-major order.  Every tile is blended (in place) over `blend_extent`
+    rows / columns with the tile above it and the tile to its left, and its first `row_limit` rows and columns are copied
+    to their place in the result (autoencoder_magvit.py:360-373 in tiled_encode, :403-416 in tiled_decode)."""
+    first = rows[0][0]
+    widths = [min(t.shape[4], row_limit) for t in rows[0]]
+    heights = [min(r[0].shape[3], row_limit) for r in rows]
+    out = torch.empty((1, first.shape[1], first.shape[2], sum(heights), sum(widths)), device=first.device, dtype=bf16)
+    r0 = 0
+    for i, row in enumerate(rows):
+        c0 = 0
+        for j, tile in enumerate(row):
+            if i > 0:
+                vae_ops.tile_blend(rows[i - 1][j], tile, blend_extent, 0)
+            if j > 0:
+                vae_ops.tile_blend(row[j - 1], tile, blend_extent, 1)
+            vae_ops.copy2d(tile, out, heights[i], widths[j], r0, c0)
+            c0 += widths[j]
+        r0 += heights[i]
+    return out
 
 
 class AutoencoderKLMagvit(nn.Module, ConfigMixinLite):
@@ -357,7 +402,7 @@ class AutoencoderKLMagvit(nn.Module, ConfigMixinLite):
         """z [C,T,h,w] planar -> [1,3,T',8h,8w]: post_quant_conv + Decoder (autoencoder_magvit.py:281-282)."""
         pq = self.post_quant_conv
         x = vae_ops.prepare_latents(z, pq.weight, pq.bias, 64, in_scale=self._latent_in_scale)
-        return self.decoder.run(x).unsqueeze(0)
+        return self.decoder.run(x, _WHOLE_FRAME).unsqueeze(0)
 
     def _tiled_decode_one(self, z: torch.Tensor) -> torch.Tensor:
         """autoencoder_magvit.py:381-448 for one batch element (z [C,T,h,w])."""
@@ -372,21 +417,7 @@ class AutoencoderKLMagvit(nn.Module, ConfigMixinLite):
             lower_right = None
         else:
             rows, lower_right = self._decode_tiles_parallel(z, coords, tl, group)
-        Tp = rows[0][0].shape[2]
-        widths = [min(t.shape[4], row_limit) for t in rows[0]]
-        heights = [min(r[0].shape[3], row_limit) for r in rows]
-        dec = torch.empty((1, rows[0][0].shape[1], Tp, sum(heights), sum(widths)), device=z.device, dtype=bf16)
-        r0 = 0
-        for i, row in enumerate(rows):
-            c0 = 0
-            for j, tile in enumerate(row):
-                if i > 0:
-                    vae_ops.tile_blend(rows[i - 1][j], tile, blend_extent, 0)
-                if j > 0:
-                    vae_ops.tile_blend(row[j - 1], tile, blend_extent, 1)
-                vae_ops.copy2d(tile, dec, heights[i], widths[j], r0, c0)
-                c0 += widths[j]
-            r0 += heights[i]
+        dec = _stitch_tiles(rows, blend_extent, row_limit)
         if lower_right is None:
             lower_right = self._decode_one(z[:, :, -tl:, -tl:].contiguous())
         vae_ops.corner_blend(lower_right, dec)
@@ -421,13 +452,17 @@ class AutoencoderKLMagvit(nn.Module, ConfigMixinLite):
             k += len(row)
         return rows, tile(len(specs) - 1).contiguous()
 
-    def _decode(self, z: torch.Tensor) -> torch.Tensor:
+    def _bf16_input(self, t: torch.Tensor, verb: str, what: str) -> torch.Tensor:
+        """The guards decode and encode share; `verb` / `what` word the errors."""
         if self.upcast_vae:
-            raise NotImplementedError("upcast_vae (fp32 decode) is not implemented: easyanimate_b200 computes in bf16")
+            raise NotImplementedError(f"upcast_vae (fp32 {verb}) is not implemented: easyanimate_b200 computes in bf16")
         if self.dtype != bf16:
             raise L.EaError("easyanimate_b200 computes in bf16: call .to(torch.bfloat16) on the module first")
-        _require_cuda(z, "latents")
-        z = z.to(bf16)
+        _require_cuda(t, what)
+        return t.to(bf16)
+
+    def _decode(self, z: torch.Tensor) -> torch.Tensor:
+        z = self._bf16_input(z, "decode", "latents")
         tl = self.tile_latent_min_size
         tiled = (self.use_tiling or self.use_tiling_decoder) and (z.shape[-1] > tl or z.shape[-2] > tl)
         if not tiled and self.strip_parallel_group is not None:
@@ -476,7 +511,7 @@ class AutoencoderKLMagvit(nn.Module, ConfigMixinLite):
             raise ValueError(f"encode needs 1 + 4m frames (the reference encodes frame 0 and then 4 frames at a time), got {x.shape[1]}")
         eye = torch.eye(cin, device=x.device, dtype=bf16)
         xin = vae_ops.prepare_latents(x, eye, torch.zeros(cin, device=x.device, dtype=bf16), 64)  # planar -> [T,H,W,64]
-        h = self.encoder.run(xin)                                   # planar [2L, T', h, w]
+        h = self.encoder.run(xin, _WHOLE_FRAME)                     # planar [2L, T', h, w]
         qc = self.quant_conv
         m = vae_ops.prepare_latents(h, qc.weight, qc.bias, h.shape[0])  # 1x1x1 conv -> channels-last [T', h, w, 2L]
         return m.permute(3, 0, 1, 2).unsqueeze(0).contiguous()
@@ -489,31 +524,12 @@ class AutoencoderKLMagvit(nn.Module, ConfigMixinLite):
         row_limit = tl - blend_extent
         rows = [[self._encode_one(x[:, :, i:i + ts, j:j + ts].contiguous()) for j in range(0, x.shape[3], overlap_size)]
                 for i in range(0, x.shape[2], overlap_size)]
-        widths = [min(t.shape[4], row_limit) for t in rows[0]]
-        heights = [min(r[0].shape[3], row_limit) for r in rows]
-        out = torch.empty((1, rows[0][0].shape[1], rows[0][0].shape[2], sum(heights), sum(widths)), device=x.device, dtype=bf16)
-        r0 = 0
-        for i, row in enumerate(rows):
-            c0 = 0
-            for j, tile in enumerate(row):
-                if i > 0:
-                    vae_ops.tile_blend(rows[i - 1][j], tile, blend_extent, 0)
-                if j > 0:
-                    vae_ops.tile_blend(row[j - 1], tile, blend_extent, 1)
-                vae_ops.copy2d(tile, out, heights[i], widths[j], r0, c0)
-                c0 += widths[j]
-            r0 += heights[i]
-        return out
+        return _stitch_tiles(rows, blend_extent, row_limit)
 
     @torch.no_grad()
     def encode(self, x: torch.Tensor, return_dict: bool = True):
         """autoencoder_magvit.py:229-269: x [B,3,T,H,W] in [-1,1] -> posterior over [B,latent,T',H/8,W/8] (T = 1 + 4m)."""
-        if self.upcast_vae:
-            raise NotImplementedError("upcast_vae (fp32 encode) is not implemented: easyanimate_b200 computes in bf16")
-        if self.dtype != bf16:
-            raise L.EaError("easyanimate_b200 computes in bf16: call .to(torch.bfloat16) on the module first")
-        _require_cuda(x, "the video")
-        x = x.to(bf16)
+        x = self._bf16_input(x, "encode", "the video")
         ts = self.tile_sample_min_size
         tiled = (self.use_tiling or self.use_tiling_encoder) and (x.shape[-1] > ts or x.shape[-2] > ts)
         outs = [(self._tiled_encode_one(xb) if tiled else self._encode_one(xb.contiguous())) for xb in x]

@@ -26,7 +26,7 @@ from typing import List, Optional
 import torch
 import torch.nn as nn
 
-from . import ops, vae_ops
+from . import vae_ops
 
 bf16 = torch.bfloat16
 
@@ -37,6 +37,9 @@ def strip_bounds(h: int, world: int) -> List[int]:
 
 
 class StripDecoder:
+    """One rank's strip of one decode: the four primitives `_Decoder.run` is written against (conv, gn, attn, upsample; see
+    autoencoder_magvit._WholeFrame for the single-GPU four) plus the communication they need."""
+
     def __init__(self, vae, group):
         import torch.distributed as dist
 
@@ -46,7 +49,7 @@ class StripDecoder:
         self.rank = dist.get_rank(group)
         self.world = dist.get_world_size(group)
         self.ranks = dist.get_process_group_ranks(group)  # global ranks, for point-to-point
-        self.stats = {"halo_bytes": 0, "gathers": 0}
+        self.bounds: List[int] = []  # rows [bounds[r], bounds[r+1]) of the current activation belong to rank r
 
     # ---- communication --------------------------------------------------------------------------------------------
     def _halo_rows(self, x: torch.Tensor):
@@ -70,12 +73,12 @@ class StripDecoder:
         if opsl:
             for w in dist.batch_isend_irecv(opsl):
                 w.wait()
-            self.stats["halo_bytes"] += top.numel() * 2 * (len(opsl) // 2)
         return top, bot
 
-    def _gather_rows(self, x: torch.Tensor, dim: int, bounds: List[int]) -> torch.Tensor:
-        """All-gather strips that differ in extent along `dim` (bounds in units of that dimension): padded to the tallest
-        strip, ONE all_gather_into_tensor, then cut back and concatenated."""
+    def _gather_rows(self, x: torch.Tensor, dim: int) -> torch.Tensor:
+        """All-gather strips that differ in extent along `dim` (the row dimension): padded to the tallest strip, ONE
+        all_gather_into_tensor, then cut back and concatenated."""
+        bounds = self.bounds
         hmax = max(bounds[r + 1] - bounds[r] for r in range(self.world))
         pad_shape = list(x.shape)
         pad_shape[dim] = hmax
@@ -84,80 +87,45 @@ class StripDecoder:
         out = torch.empty([self.world * pad_shape[0]] + pad_shape[1:], device=x.device, dtype=x.dtype)  # concatenated along dim 0
         self.dist.all_gather_into_tensor(out, buf, group=self.group)
         out = out.view([self.world] + pad_shape)
-        self.stats["gathers"] += 1
         return torch.cat([out[r].narrow(dim, 0, bounds[r + 1] - bounds[r]) for r in range(self.world)], dim=dim)
 
-    # ---- layers ---------------------------------------------------------------------------------------------------
+    # ---- the four primitives --------------------------------------------------------------------------------------
     def conv(self, c, x: torch.Tensor, **kw) -> torch.Tensor:
         top, bot = self._halo_rows(x)
         xe = torch.cat([top, x, bot], dim=1)  # data movement only: [T, Hs+2, W, C]
         return vae_ops.conv3d_causal(xe, c.packed(), c.bias, c.out_channels, out_row0=1, out_rows=x.shape[1], **kw)
 
-    def gn(self, norm: nn.GroupNorm, x: torch.Tensor, H_full: int, silu: bool) -> torch.Tensor:
+    def gn(self, norm: nn.GroupNorm, x: torch.Tensor, silu: bool) -> torch.Tensor:
         T, Hs, W, Cc = x.shape
         G = norm.num_groups
         sums = vae_ops.groupnorm_sums(x, G)
         all_sums = torch.empty((self.world * T, G, 2), device=x.device, dtype=torch.float64)
         self.dist.all_gather_into_tensor(all_sums, sums, group=self.group)
         all_sums = all_sums.view(self.world, T, G, 2)
-        count = float(H_full) * W * (Cc // G)
+        count = float(self.bounds[-1]) * W * (Cc // G)  # of the whole frame
         return vae_ops.groupnorm_from_sums(x, all_sums, count, norm.weight, norm.bias, G, norm.eps, silu)
 
-    def res(self, r, x: torch.Tensor, H_full: int) -> torch.Tensor:
-        T, Hs, W, Cin = x.shape
-        if isinstance(r.shortcut, nn.Identity):
-            sc = x
-        else:
-            co = r.shortcut.out_channels
-            sc = ops.gemm(x.view(T * Hs * W, Cin), r.shortcut.weight.view(co, Cin), r.shortcut.bias).view(T, Hs, W, co)
-        h = self.gn(r.norm1, x, H_full, True)
-        h = self.conv(r.conv1, h)
-        h = self.gn(r.norm2, h, H_full, True)
-        return self.conv(r.conv2, h, residual=sc)
+    def attn(self, a, n: torch.Tensor, x: torch.Tensor) -> torch.Tensor:
+        W = x.shape[2]
+        n_full = self._gather_rows(n, 1).contiguous()  # [T, H, W, C]
+        return a.attend(n_full, x, q_rows=(self.bounds[self.rank] * W, self.bounds[self.rank + 1] * W))
 
-    def attn(self, a, x: torch.Tensor, bounds: List[int]) -> torch.Tensor:
-        T, Hs, W, Cc = x.shape
-        H_full = bounds[-1]
-        n = self.gn(a.group_norm, x, H_full, False)
-        n_full = self._gather_rows(n, 1, bounds).contiguous()  # [T, H, W, C]
-        w, b = a._qkv()
-        r0, r1 = bounds[self.rank], bounds[self.rank + 1]
-        out = vae_ops.spatial_attention(n_full.view(T * H_full * W, Cc), w, b, a.to_out.weight, a.to_out.bias,
-                                        x.view(T * Hs * W, Cc), T, a.scale, q_rows=(r0 * W, r1 * W))
-        return out.view(T, Hs, W, Cc)
+    def upsample(self, x: torch.Tensor) -> torch.Tensor:
+        self.bounds = [2 * b for b in self.bounds]
+        return vae_ops.upsample2x(x)
 
     # ---- the decoder ----------------------------------------------------------------------------------------------
     def decode(self, z: torch.Tensor, in_scale: float = 1.0) -> torch.Tensor:
         """z [C,T,h,w] planar (the SAME latent on every rank) -> [1,3,T',8h,8w] on every rank."""
-        vae, dec = self.vae, self.vae.decoder
         h = z.shape[2]
         if h < self.world:
             raise ValueError(f"strip-parallel decode needs at least one latent row per rank ({h} rows, {self.world} ranks)")
-        lat = strip_bounds(h, self.world)
-        r0, r1 = lat[self.rank], lat[self.rank + 1]
-        pq = vae.post_quant_conv
+        self.bounds = strip_bounds(h, self.world)
+        r0, r1 = self.bounds[self.rank], self.bounds[self.rank + 1]
+        pq = self.vae.post_quant_conv
         x = vae_ops.prepare_latents(z[:, :, r0:r1].contiguous(), pq.weight, pq.bias, 64, in_scale=in_scale)
-        scale = 1
-        H = h
-        x = self.conv(dec.conv_in, x)
-        mid = dec.mid_block
-        x = self.res(mid.convs[0], x, H)
-        for a, r in zip(mid.attentions, mid.convs[1:]):
-            if a is not None:
-                x = self.attn(a, x, [b * scale for b in lat])
-            x = self.res(r, x, H)
-        for up in dec.up_blocks:
-            for r in up.convs:
-                x = self.res(r, x, H)
-            if up.upsampler is not None:
-                x = vae_ops.upsample2x(x)
-                scale *= 2
-                H *= 2
-                x = self.conv(up.upsampler.conv, x, dup_frames=up.upsampler.temporal and x.shape[0] > 1)
-        x = self.gn(dec.conv_norm_out, x, H, True)
-        y = self.conv(dec.conv_out, x, out_planar=True)  # [3, T', 8 hs, 8 w]
-        full = self._gather_rows(y, 2, [b * scale for b in lat])
-        return full.unsqueeze(0)
+        y = self.vae.decoder.run(x, self)  # [3, T', 8 hs, 8 w]; the up-samplers have scaled the bounds with it
+        return self._gather_rows(y, 2).unsqueeze(0)
 
 
 def decode_strips(vae, z: torch.Tensor, group, in_scale: float = 1.0) -> torch.Tensor:

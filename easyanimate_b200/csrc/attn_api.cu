@@ -3,13 +3,12 @@
 #include "../../include/ea_b200.h"
 
 namespace ea {
-int launch_attn6(const ea_attn_args* g, cudaStream_t stream);
+int launch_attn6(const ea_attn_args* g, void* stream);
 }  // namespace ea
 
 extern "C" int ea_attn_generations(void) { return 1 << 6; }
 
-extern "C" int ea_attn_fwd(const ea_attn_args* g, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+extern "C" int ea_attn_fwd(const ea_attn_args* g, void* stream) {
   EA_REQUIRE(g && g->q && g->k && g->v, "ea_attn_fwd: null pointer");
   EA_REQUIRE(g->B > 0 && g->H > 0 && g->S > 0, "ea_attn_fwd: empty problem");
   EA_REQUIRE(g->head_dim == 64, "ea_attn_fwd: head_dim must be 64");

@@ -12,9 +12,6 @@
 #include "../../include/ea_b200.h"
 
 namespace ea {
-
-extern void count_launch();
-
 namespace a6 {
 
 constexpr int kQT = 128;
@@ -239,7 +236,7 @@ attn6_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__
   }
 }
 
-static int launch(const ea_attn_args* g, cudaStream_t stream) {
+static int launch(const ea_attn_args* g, void* stream) {
   const int64_t BH = g->B * g->H;
   CUtensorMap tq, tk, tv;
   uint64_t dims[3] = {(uint64_t)kHD, (uint64_t)g->S, (uint64_t)BH};
@@ -272,17 +269,15 @@ static int launch(const ea_attn_args* g, cudaStream_t stream) {
   static ::ea::PerDeviceFlag smem_done;
   rc = set_max_dynamic_smem(reinterpret_cast<const void*>(attn6_kernel), kTotal, smem_done, "attn6_kernel");
   if (rc) return rc;
-  dim3 grid((unsigned)((g->S + kQT - 1) / kQT), (unsigned)BH);
-  attn6_kernel<<<grid, kThreads, kTotal, stream>>>(tq, tk, tv, p);
-  count_launch();
-  return check_launch("attn6_kernel");
+  return ea::launch(attn6_kernel, dim3(grid_1d(g->S, kQT), (unsigned)BH), kThreads, kTotal, stream, "attn6_kernel", tq, tk,
+                    tv, p);
 }
 
 }  // namespace a6
 
 // One kernel on sm_90a: the exponential-split (bits 4-6), truncated-P (0x800) and three-tile layout (0x2000) selections of
 // ea_attn_args.variant are accepted and all run it.
-int launch_attn6(const ea_attn_args* g, cudaStream_t stream) {
+int launch_attn6(const ea_attn_args* g, void* stream) {
   return a6::launch(g, stream);
 }
 

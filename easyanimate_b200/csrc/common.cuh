@@ -30,16 +30,27 @@ EA_DEVICE float2 unpack_bf16x2(uint32_t u) {
   return __bfloat1622float2(v);
 }
 
+// The 8 bf16 of one 16-byte vector as floats, and back (round to nearest even). `u` is taken by value: bound to a
+// reference into global memory, the compiler splits the 16-byte load of the caller into four 4-byte loads.
+EA_DEVICE void unpack_bf16x8(uint4 u, float* f) {
+  const float2 f0 = unpack_bf16x2(u.x), f1 = unpack_bf16x2(u.y), f2 = unpack_bf16x2(u.z), f3 = unpack_bf16x2(u.w);
+  f[0] = f0.x; f[1] = f0.y; f[2] = f1.x; f[3] = f1.y;
+  f[4] = f2.x; f[5] = f2.y; f[6] = f3.x; f[7] = f3.y;
+}
+EA_DEVICE uint4 pack_bf16x8(const float* f) {
+  return make_uint4(pack_bf16x2(f[0], f[1]), pack_bf16x2(f[2], f[3]), pack_bf16x2(f[4], f[5]), pack_bf16x2(f[6], f[7]));
+}
+
 // x[j] += src[j] for j < N (N a multiple of 8; src 16-byte aligned, read through the read-only cache)
 template <int N>
 EA_DEVICE void add_bf16(float* x, const bf16* src) {
   const uint4* p = reinterpret_cast<const uint4*>(src);
 #pragma unroll
   for (int j = 0; j < N / 8; ++j) {
-    uint4 b = __ldg(p + j);
-    float2 f0 = unpack_bf16x2(b.x), f1 = unpack_bf16x2(b.y), f2 = unpack_bf16x2(b.z), f3 = unpack_bf16x2(b.w);
-    x[j * 8 + 0] += f0.x; x[j * 8 + 1] += f0.y; x[j * 8 + 2] += f1.x; x[j * 8 + 3] += f1.y;
-    x[j * 8 + 4] += f2.x; x[j * 8 + 5] += f2.y; x[j * 8 + 6] += f3.x; x[j * 8 + 7] += f3.y;
+    float f[8];
+    unpack_bf16x8(__ldg(p + j), f);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) x[j * 8 + k] += f[k];
   }
 }
 
@@ -47,14 +58,19 @@ EA_DEVICE void add_bf16(float* x, const bf16* src) {
 template <int N>
 EA_DEVICE void store_bf16(bf16* dst, const float* x) {
 #pragma unroll
-  for (int j = 0; j < N / 8; ++j) {
-    uint4 w;
-    w.x = pack_bf16x2(x[j * 8 + 0], x[j * 8 + 1]);
-    w.y = pack_bf16x2(x[j * 8 + 2], x[j * 8 + 3]);
-    w.z = pack_bf16x2(x[j * 8 + 4], x[j * 8 + 5]);
-    w.w = pack_bf16x2(x[j * 8 + 6], x[j * 8 + 7]);
-    reinterpret_cast<uint4*>(dst)[j] = w;
-  }
+  for (int j = 0; j < N / 8; ++j) reinterpret_cast<uint4*>(dst)[j] = pack_bf16x8(x + j * 8);
+}
+
+// Butterfly reductions over the 32 lanes of a warp (xor offsets 16, 8, 4, 2, 1): every lane gets the result.
+EA_DEVICE float warp_sum(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+EA_DEVICE float warp_max(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
 }
 
 // A kernel that waits on an mbarrier which never completes would hang the GPU box; every wait is

@@ -112,7 +112,7 @@ conv3d_tc_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_consta
 }
 
 template <int BN>
-static int launch_conv(const ea_conv3d_args* g, cudaStream_t stream) {
+static int launch_conv(const ea_conv3d_args* g, void* stream) {
   ConvDevArgs p{};
   p.st = g->stride_t == 2 ? 2 : 1;
   p.shw = g->stride_hw == 2 ? 2 : 1;
@@ -168,8 +168,7 @@ static int launch_conv(const ea_conv3d_args* g, cudaStream_t stream) {
 
 using namespace ea;
 
-extern "C" int ea_conv3d_causal(const ea_conv3d_args* g, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+extern "C" int ea_conv3d_causal(const ea_conv3d_args* g, void* stream) {
   EA_REQUIRE(g && g->x && g->w && g->bias && g->out, "ea_conv3d_causal: null pointer");
   EA_REQUIRE(g->T > 0 && g->H > 0 && g->W > 0, "ea_conv3d_causal: empty input");
   EA_REQUIRE(g->Cin > 0 && g->Cin % 64 == 0, "ea_conv3d_causal: Cin must be a multiple of 64 (pad the channels)");

@@ -2,19 +2,13 @@
 // patchify / unpatchify, CFG combine + Euler step.  One warp per token row, 16-byte vector loads/stores, values
 // held in registers so every tensor is read once and written once.  bf16 rounding points follow the reference's
 // op-by-op bf16 execution (each torch op materialises a bf16 tensor).
+#include <algorithm>
+
 #include "common.cuh"
 #include "host.h"
 #include "../../include/ea_b200.h"
 
 namespace ea {
-
-extern void count_launch();
-
-EA_DEVICE float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
 
 struct LnArgs {
   const bf16* x;
@@ -48,10 +42,7 @@ __global__ void __launch_bounds__(256) ln_modulate_kernel(const LnArgs a) {
   for (int i = 0; i < NI; ++i) {
     const int vi = lane + 32 * i;
     if (vi < nvec) {
-      uint4 u = xp[vi];
-      float2 f0 = unpack_bf16x2(u.x), f1 = unpack_bf16x2(u.y), f2 = unpack_bf16x2(u.z), f3 = unpack_bf16x2(u.w);
-      v[i][0] = f0.x; v[i][1] = f0.y; v[i][2] = f1.x; v[i][3] = f1.y;
-      v[i][4] = f2.x; v[i][5] = f2.y; v[i][6] = f3.x; v[i][7] = f3.y;
+      unpack_bf16x8(xp[vi], v[i]);
     } else {
 #pragma unroll
       for (int j = 0; j < 8; ++j) v[i][j] = 0.f;
@@ -85,17 +76,8 @@ __global__ void __launch_bounds__(256) ln_modulate_kernel(const LnArgs a) {
       if (vi < nvec) {
         float wv[8], bv[8];
         if (w != nullptr) {
-          uint4 wu = __ldg(reinterpret_cast<const uint4*>(w) + vi);
-          uint4 bu = __ldg(reinterpret_cast<const uint4*>(b) + vi);
-          float2 t;
-          t = unpack_bf16x2(wu.x); wv[0] = t.x; wv[1] = t.y;
-          t = unpack_bf16x2(wu.y); wv[2] = t.x; wv[3] = t.y;
-          t = unpack_bf16x2(wu.z); wv[4] = t.x; wv[5] = t.y;
-          t = unpack_bf16x2(wu.w); wv[6] = t.x; wv[7] = t.y;
-          t = unpack_bf16x2(bu.x); bv[0] = t.x; bv[1] = t.y;
-          t = unpack_bf16x2(bu.y); bv[2] = t.x; bv[3] = t.y;
-          t = unpack_bf16x2(bu.z); bv[4] = t.x; bv[5] = t.y;
-          t = unpack_bf16x2(bu.w); bv[6] = t.x; bv[7] = t.y;
+          unpack_bf16x8(__ldg(reinterpret_cast<const uint4*>(w) + vi), wv);
+          unpack_bf16x8(__ldg(reinterpret_cast<const uint4*>(b) + vi), bv);
         } else {
 #pragma unroll
           for (int j = 0; j < 8; ++j) { wv[j] = 1.f; bv[j] = 0.f; }
@@ -131,12 +113,7 @@ __global__ void __launch_bounds__(256) ln_modulate_kernel(const LnArgs a) {
           v[i][2 * t + 1] = m1 + hf.y;
         }
       }
-      uint4 o;
-      o.x = pack_bf16x2(v[i][0], v[i][1]);
-      o.y = pack_bf16x2(v[i][2], v[i][3]);
-      o.z = pack_bf16x2(v[i][4], v[i][5]);
-      o.w = pack_bf16x2(v[i][6], v[i][7]);
-      yp[vi] = o;
+      yp[vi] = pack_bf16x8(v[i]);
     }
   }
 }
@@ -163,10 +140,7 @@ __global__ void __launch_bounds__(256) rmsnorm_kernel(const RmsArgs a) {
   for (int i = 0; i < NI; ++i) {
     const int vi = lane + 32 * i;
     if (vi < nvec) {
-      uint4 u = xp[vi];
-      float2 f0 = unpack_bf16x2(u.x), f1 = unpack_bf16x2(u.y), f2 = unpack_bf16x2(u.z), f3 = unpack_bf16x2(u.w);
-      v[i][0] = f0.x; v[i][1] = f0.y; v[i][2] = f1.x; v[i][3] = f1.y;
-      v[i][4] = f2.x; v[i][5] = f2.y; v[i][6] = f3.x; v[i][7] = f3.y;
+      unpack_bf16x8(xp[vi], v[i]);
 #pragma unroll
       for (int j = 0; j < 8; ++j) s += v[i][j] * v[i][j];
     }
@@ -233,13 +207,8 @@ __global__ void __launch_bounds__(256) skinny_linear_kernel(const bf16* __restri
   const uint4* wp = reinterpret_cast<const uint4*>(w + (int64_t)n * K);
   const int nvec = K >> 3;
   for (int vi = lane; vi < nvec; vi += 32) {
-    uint4 u = __ldg(wp + vi);
     float wv[8];
-    float2 t;
-    t = unpack_bf16x2(u.x); wv[0] = t.x; wv[1] = t.y;
-    t = unpack_bf16x2(u.y); wv[2] = t.x; wv[3] = t.y;
-    t = unpack_bf16x2(u.z); wv[4] = t.x; wv[5] = t.y;
-    t = unpack_bf16x2(u.w); wv[6] = t.x; wv[7] = t.y;
+    unpack_bf16x8(__ldg(wp + vi), wv);
 #pragma unroll
     for (int m = 0; m < MAXM; ++m) {
       if (m < M) {
@@ -261,6 +230,19 @@ __global__ void __launch_bounds__(256) skinny_linear_kernel(const bf16* __restri
   }
 }
 
+// idx -> (b, c, f, hh, ww) of a [B][C][F][Hp][Wp] index space, ww fastest
+struct PatchPos {
+  int b, c, f, hh, ww;
+};
+EA_DEVICE PatchPos patch_pos(int64_t idx, int C, int F, int Hp, int Wp) {
+  const int ww = idx % Wp;
+  int64_t r = idx / Wp;
+  const int hh = r % Hp; r /= Hp;
+  const int f = r % F; r /= F;
+  const int c = r % C; r /= C;
+  return {(int)r, c, f, hh, ww};
+}
+
 // A[(b,f,hh,ww), c*4 + ph*2 + pw] = cat(x, x2)[b, c, f, 2hh+ph, 2ww+pw];  columns >= 4*C are zero (K padding)
 __global__ void patchify_kernel(const bf16* __restrict__ x, const bf16* __restrict__ x2, bf16* __restrict__ a, int B,
                                 int C1, int C2, int F, int H, int W, int ldk) {
@@ -270,12 +252,7 @@ __global__ void patchify_kernel(const bf16* __restrict__ x, const bf16* __restri
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= total) return;
   // thread -> (row, c): ww fastest so reads of x rows are (2-element) coalesced
-  const int ww = idx % Wp;
-  int64_t r = idx / Wp;
-  const int hh = r % Hp; r /= Hp;
-  const int f = r % F; r /= F;
-  const int c = r % C; r /= C;
-  const int b = (int)r;
+  const auto [b, c, f, hh, ww] = patch_pos(idx, C, F, Hp, Wp);
   const bf16* src;
   int cc, CC;
   if (c < C1) { src = x; cc = c; CC = C1; } else { src = x2; cc = c - C1; CC = C2; }
@@ -300,12 +277,7 @@ __global__ void unpatchify_kernel(const bf16* __restrict__ y, bf16* __restrict__
   const int64_t total = (int64_t)B * C * F * Hp * Wp;
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= total) return;
-  const int ww = idx % Wp;
-  int64_t r = idx / Wp;
-  const int hh = r % Hp; r /= Hp;
-  const int f = r % F; r /= F;
-  const int c = r % C; r /= C;
-  const int b = (int)r;
+  const auto [b, c, f, hh, ww] = patch_pos(idx, C, F, Hp, Wp);
   const int64_t row = (((int64_t)b * F + f) * Hp + hh) * Wp + ww;
   const uint2 v = *reinterpret_cast<const uint2*>(y + row * ldy + c * 4);
   const int64_t base = ((((int64_t)b * C + c) * F + f) * H + 2 * hh) * W + 2 * ww;
@@ -333,153 +305,8 @@ __global__ void cfg_euler_kernel(const bf16* __restrict__ pred_uncond, const bf1
   *reinterpret_cast<uint32_t*>(x_out + i) = pack_bf16x2(o0, o1);
 }
 
-template <int NI>
-static void launch_ln(const LnArgs& a, cudaStream_t s) {
-  const int warps_per_block = 8;
-  const int64_t blocks = (a.rows + warps_per_block - 1) / warps_per_block;
-  ln_modulate_kernel<NI><<<(unsigned)blocks, warps_per_block * 32, 0, s>>>(a);
-}
-template <int NI>
-static void launch_rms(const RmsArgs& a, cudaStream_t s) {
-  const int warps_per_block = 8;
-  const int64_t blocks = (a.rows + warps_per_block - 1) / warps_per_block;
-  rmsnorm_kernel<NI><<<(unsigned)blocks, warps_per_block * 32, 0, s>>>(a);
-}
-
-}  // namespace ea
-
-using namespace ea;
-
-#define EA_DISPATCH_NI(ni, CALL)                                                         \
-  switch (ni) {                                                                          \
-    case 1: CALL(1); break;   case 2: CALL(2); break;   case 3: CALL(3); break;          \
-    case 4: CALL(4); break;   case 5: CALL(5); break;   case 6: CALL(6); break;          \
-    case 7: CALL(7); break;   case 8: CALL(8); break;   case 9: CALL(9); break;          \
-    case 10: CALL(10); break; case 11: CALL(11); break; case 12: CALL(12); break;        \
-    case 13: CALL(13); break; case 14: CALL(14); break; case 15: CALL(15); break;        \
-    case 16: CALL(16); break;                                                            \
-    default: return fail(EA_ERR_INVALID, "feature dimension larger than 4096 is not supported"); \
-  }
-
-extern "C" int ea_layernorm_modulate(const ea_ln_args* g, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  EA_REQUIRE(g && g->x && g->y, "ea_layernorm_modulate: null pointer");
-  EA_REQUIRE(g->rows > 0 && g->d > 0 && g->d % 8 == 0, "ea_layernorm_modulate: d must be a positive multiple of 8");
-  EA_REQUIRE(g->ldx % 8 == 0 && g->ldy % 8 == 0, "ea_layernorm_modulate: row strides must be multiples of 8");
-  EA_REQUIRE((g->w == nullptr) == (g->b == nullptr), "ea_layernorm_modulate: weight and bias must come together");
-  EA_REQUIRE((g->pre_w == nullptr) == (g->pre_b == nullptr), "ea_layernorm_modulate: pre weight/bias must come together");
-  EA_REQUIRE((g->shift == nullptr) == (g->scale == nullptr), "ea_layernorm_modulate: shift and scale must come together");
-  LnArgs a{};
-  a.x = (const bf16*)g->x; a.y = (bf16*)g->y; a.rows = g->rows; a.d = (int)g->d;
-  a.ldx = g->ldx; a.ldy = g->ldy;
-  a.rows_per_batch = (int)(g->rows_per_batch > 0 ? g->rows_per_batch : g->rows);
-  a.pre_w = (const bf16*)g->pre_w; a.pre_b = (const bf16*)g->pre_b; a.pre_eps = g->pre_eps;
-  a.w = (const bf16*)g->w; a.b = (const bf16*)g->b; a.eps = g->eps;
-  a.shift = (const bf16*)g->shift; a.scale = (const bf16*)g->scale; a.mod_stride = g->mod_stride;
-  const int ni = (int)((g->d + 255) / 256);
-#define CALL(n) launch_ln<n>(a, stream)
-  EA_DISPATCH_NI(ni, CALL)
-#undef CALL
-  count_launch();
-  return check_launch("ln_modulate_kernel");
-}
-
-extern "C" int ea_rmsnorm(const ea_rmsnorm_args* g, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  EA_REQUIRE(g && g->x && g->y && g->w, "ea_rmsnorm: null pointer");
-  EA_REQUIRE(g->rows > 0 && g->d > 0 && g->d % 8 == 0, "ea_rmsnorm: d must be a positive multiple of 8");
-  RmsArgs a{(const bf16*)g->x, (bf16*)g->y, (const bf16*)g->w, g->rows, (int)g->d, g->eps};
-  const int ni = (int)((g->d + 255) / 256);
-#define CALL(n) launch_rms<n>(a, stream)
-  EA_DISPATCH_NI(ni, CALL)
-#undef CALL
-  count_launch();
-  return check_launch("rmsnorm_kernel");
-}
-
-extern "C" int ea_timestep_embedding(const void* t, void* out, int64_t B, int64_t dim, float freq_shift,
-                                     int32_t flip_sin_to_cos, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  EA_REQUIRE(t && out && B > 0 && dim > 0 && dim % 2 == 0, "ea_timestep_embedding: bad arguments");
-  const int n = (int)(B * dim / 2);
-  timestep_embedding_kernel<<<(n + 255) / 256, 256, 0, stream>>>((const bf16*)t, (bf16*)out, (int)B, (int)dim,
-                                                                freq_shift, flip_sin_to_cos);
-  count_launch();
-  return check_launch("timestep_embedding_kernel");
-}
-
-extern "C" int ea_skinny_linear(const ea_skinny_linear_args* g, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  EA_REQUIRE(g && g->x && g->w && g->out, "ea_skinny_linear: null pointer");
-  EA_REQUIRE(g->M >= 1 && g->M <= 8, "ea_skinny_linear: M must be in [1,8]");
-  EA_REQUIRE(g->K > 0 && g->K % 8 == 0 && g->N > 0, "ea_skinny_linear: K must be a positive multiple of 8");
-  const size_t smem = (size_t)g->M * g->K * sizeof(float);
-  EA_REQUIRE(smem <= 96 * 1024, "ea_skinny_linear: M*K too large for the shared-memory input stage");
-  auto kern = skinny_linear_kernel<8>;
-  static ::ea::PerDeviceFlag attr_flag;
-  const int attr_dev = ::ea::current_device();
-  if (!attr_flag.get(attr_dev)) {
-    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
-    attr_flag.set(attr_dev);
-  }
-  const int warps = 8;
-  kern<<<(unsigned)((g->N + warps - 1) / warps), warps * 32, smem, stream>>>(
-      (const bf16*)g->x, (const bf16*)g->w, (const bf16*)g->bias, (bf16*)g->out, (int)g->M, (int)g->N, (int)g->K,
-      g->act_in, g->act_out);
-  count_launch();
-  return check_launch("skinny_linear_kernel");
-}
-
-extern "C" int ea_patchify(const void* x, const void* x2, void* a, int64_t B, int64_t C1, int64_t C2, int64_t F,
-                           int64_t H, int64_t W, int64_t ldk, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  EA_REQUIRE(x && a, "ea_patchify: null pointer");
-  EA_REQUIRE(C2 == 0 || x2 != nullptr, "ea_patchify: second source missing");
-  EA_REQUIRE(H % 2 == 0 && W % 2 == 0, "ea_patchify: H and W must be even (patch size 2)");
-  EA_REQUIRE(ldk >= 4 * (C1 + C2) && ldk % 8 == 0, "ea_patchify: ldk must be a multiple of 8 and >= 4*C");
-  const int64_t rows = B * F * (H / 2) * (W / 2);
-  const int64_t total = rows * (C1 + C2);
-  patchify_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>((const bf16*)x, (const bf16*)x2, (bf16*)a, (int)B,
-                                                                      (int)C1, (int)C2, (int)F, (int)H, (int)W, (int)ldk);
-  count_launch();
-  const int kvalid = (int)(4 * (C1 + C2));
-  if (ldk > kvalid) {
-    const int64_t tp = rows * (ldk - kvalid);
-    patchify_pad_kernel<<<(unsigned)((tp + 255) / 256), 256, 0, stream>>>((bf16*)a, rows, kvalid, (int)ldk);
-    count_launch();
-  }
-  return check_launch("patchify_kernel");
-}
-
-extern "C" int ea_unpatchify(const void* y, void* out, int64_t B, int64_t C, int64_t F, int64_t H, int64_t W,
-                             int64_t ldy, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  EA_REQUIRE(y && out, "ea_unpatchify: null pointer");
-  EA_REQUIRE(H % 2 == 0 && W % 2 == 0 && ldy >= 4 * C && ldy % 4 == 0, "ea_unpatchify: bad shape");
-  const int64_t total = B * C * F * (H / 2) * (W / 2);
-  unpatchify_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>((const bf16*)y, (bf16*)out, (int)B, (int)C,
-                                                                        (int)F, (int)H, (int)W, (int)ldy);
-  count_launch();
-  return check_launch("unpatchify_kernel");
-}
-
-extern "C" int ea_cfg_euler_step(const void* pred_uncond, const void* pred_text, const void* x, void* x_out, int64_t n,
-                                 float guidance_scale, int32_t use_cfg, float sigma, float sigma_next, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  EA_REQUIRE(pred_uncond && x && x_out, "ea_cfg_euler_step: null pointer");
-  EA_REQUIRE(!use_cfg || pred_text, "ea_cfg_euler_step: CFG needs the text-conditioned prediction");
-  EA_REQUIRE(n > 0 && n % 2 == 0, "ea_cfg_euler_step: element count must be even");
-  const float dt = sigma_next - sigma;  // fp32 subtraction of fp32 sigmas, as the scheduler does
-  cfg_euler_kernel<<<(unsigned)((n / 2 + 255) / 256), 256, 0, stream>>>((const bf16*)pred_uncond, (const bf16*)pred_text,
-                                                                       (const bf16*)x, (bf16*)x_out, n, guidance_scale,
-                                                                       use_cfg, dt);
-  count_launch();
-  return check_launch("cfg_euler_kernel");
-}
-
 // ---- TeaCache support (transformer3d.py:90-121,1563-1636): relative-L1 change of the block-0 modulated input and
 //      the cached-residual add/sub, kept on the device (the reference round-trips both tensors through the CPU).
-namespace ea {
 __global__ void __launch_bounds__(256) l1_sums_kernel(const bf16* __restrict__ cur, const bf16* __restrict__ prev,
                                                       double* __restrict__ sums, int64_t n) {
   float s_diff = 0.f, s_prev = 0.f;
@@ -543,35 +370,130 @@ __global__ void dequant_e4m3_kernel(const uint8_t* __restrict__ w8, bf16* __rest
     for (int64_t i = i0; i < n; ++i) w16[i] = __ushort_as_bfloat16(lut[w8[i]]);
   }
 }
+
 }  // namespace ea
 
-extern "C" int ea_dequant_e4m3(const void* w8, void* w16, int64_t n, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+using namespace ea;
+
+#define EA_DISPATCH_NI(ni, CALL)                                                         \
+  switch (ni) {                                                                          \
+    case 1: CALL(1); break;   case 2: CALL(2); break;   case 3: CALL(3); break;          \
+    case 4: CALL(4); break;   case 5: CALL(5); break;   case 6: CALL(6); break;          \
+    case 7: CALL(7); break;   case 8: CALL(8); break;   case 9: CALL(9); break;          \
+    case 10: CALL(10); break; case 11: CALL(11); break; case 12: CALL(12); break;        \
+    case 13: CALL(13); break; case 14: CALL(14); break; case 15: CALL(15); break;        \
+    case 16: CALL(16); break;                                                            \
+    default: return fail(EA_ERR_INVALID, "feature dimension larger than 4096 is not supported"); \
+  }
+
+// The LayerNorm and RMSNorm kernels take one warp per row: 8 rows per block of 256 threads.
+extern "C" int ea_layernorm_modulate(const ea_ln_args* g, void* stream) {
+  EA_REQUIRE(g && g->x && g->y, "ea_layernorm_modulate: null pointer");
+  EA_REQUIRE(g->rows > 0 && g->d > 0 && g->d % 8 == 0, "ea_layernorm_modulate: d must be a positive multiple of 8");
+  EA_REQUIRE(g->ldx % 8 == 0 && g->ldy % 8 == 0, "ea_layernorm_modulate: row strides must be multiples of 8");
+  EA_REQUIRE((g->w == nullptr) == (g->b == nullptr), "ea_layernorm_modulate: weight and bias must come together");
+  EA_REQUIRE((g->pre_w == nullptr) == (g->pre_b == nullptr), "ea_layernorm_modulate: pre weight/bias must come together");
+  EA_REQUIRE((g->shift == nullptr) == (g->scale == nullptr), "ea_layernorm_modulate: shift and scale must come together");
+  LnArgs a{};
+  a.x = (const bf16*)g->x; a.y = (bf16*)g->y; a.rows = g->rows; a.d = (int)g->d;
+  a.ldx = g->ldx; a.ldy = g->ldy;
+  a.rows_per_batch = (int)(g->rows_per_batch > 0 ? g->rows_per_batch : g->rows);
+  a.pre_w = (const bf16*)g->pre_w; a.pre_b = (const bf16*)g->pre_b; a.pre_eps = g->pre_eps;
+  a.w = (const bf16*)g->w; a.b = (const bf16*)g->b; a.eps = g->eps;
+  a.shift = (const bf16*)g->shift; a.scale = (const bf16*)g->scale; a.mod_stride = g->mod_stride;
+  const int ni = (int)((g->d + 255) / 256);
+#define CALL(n) return launch(ln_modulate_kernel<n>, grid_1d(a.rows, 8), 256, 0, stream, "ln_modulate_kernel", a)
+  EA_DISPATCH_NI(ni, CALL)
+#undef CALL
+}
+
+extern "C" int ea_rmsnorm(const ea_rmsnorm_args* g, void* stream) {
+  EA_REQUIRE(g && g->x && g->y && g->w, "ea_rmsnorm: null pointer");
+  EA_REQUIRE(g->rows > 0 && g->d > 0 && g->d % 8 == 0, "ea_rmsnorm: d must be a positive multiple of 8");
+  RmsArgs a{(const bf16*)g->x, (bf16*)g->y, (const bf16*)g->w, g->rows, (int)g->d, g->eps};
+  const int ni = (int)((g->d + 255) / 256);
+#define CALL(n) return launch(rmsnorm_kernel<n>, grid_1d(a.rows, 8), 256, 0, stream, "rmsnorm_kernel", a)
+  EA_DISPATCH_NI(ni, CALL)
+#undef CALL
+}
+
+extern "C" int ea_timestep_embedding(const void* t, void* out, int64_t B, int64_t dim, float freq_shift,
+                                     int32_t flip_sin_to_cos, void* stream) {
+  EA_REQUIRE(t && out && B > 0 && dim > 0 && dim % 2 == 0, "ea_timestep_embedding: bad arguments");
+  const int n = (int)(B * dim / 2);
+  return launch(timestep_embedding_kernel, grid_1d(n, 256), 256, 0, stream, "timestep_embedding_kernel", (const bf16*)t,
+                (bf16*)out, (int)B, (int)dim, freq_shift, flip_sin_to_cos);
+}
+
+extern "C" int ea_skinny_linear(const ea_skinny_linear_args* g, void* stream) {
+  EA_REQUIRE(g && g->x && g->w && g->out, "ea_skinny_linear: null pointer");
+  EA_REQUIRE(g->M >= 1 && g->M <= 8, "ea_skinny_linear: M must be in [1,8]");
+  EA_REQUIRE(g->K > 0 && g->K % 8 == 0 && g->N > 0, "ea_skinny_linear: K must be a positive multiple of 8");
+  const size_t smem = (size_t)g->M * g->K * sizeof(float);
+  EA_REQUIRE(smem <= 96 * 1024, "ea_skinny_linear: M*K too large for the shared-memory input stage");
+  static PerDeviceFlag smem_done;
+  const int rc = set_max_dynamic_smem(reinterpret_cast<const void*>(skinny_linear_kernel<8>), 96 * 1024, smem_done,
+                                      "skinny_linear_kernel");
+  if (rc) return rc;
+  // one warp per output column, 8 per block
+  return launch(skinny_linear_kernel<8>, grid_1d(g->N, 8), 256, smem, stream, "skinny_linear_kernel", (const bf16*)g->x,
+                (const bf16*)g->w, (const bf16*)g->bias, (bf16*)g->out, (int)g->M, (int)g->N, (int)g->K, g->act_in,
+                g->act_out);
+}
+
+extern "C" int ea_patchify(const void* x, const void* x2, void* a, int64_t B, int64_t C1, int64_t C2, int64_t F,
+                           int64_t H, int64_t W, int64_t ldk, void* stream) {
+  EA_REQUIRE(x && a, "ea_patchify: null pointer");
+  EA_REQUIRE(C2 == 0 || x2 != nullptr, "ea_patchify: second source missing");
+  EA_REQUIRE(H % 2 == 0 && W % 2 == 0, "ea_patchify: H and W must be even (patch size 2)");
+  EA_REQUIRE(ldk >= 4 * (C1 + C2) && ldk % 8 == 0, "ea_patchify: ldk must be a multiple of 8 and >= 4*C");
+  const int64_t rows = B * F * (H / 2) * (W / 2);
+  int rc = launch(patchify_kernel, grid_1d(rows * (C1 + C2), 256), 256, 0, stream, "patchify_kernel", (const bf16*)x,
+                  (const bf16*)x2, (bf16*)a, (int)B, (int)C1, (int)C2, (int)F, (int)H, (int)W, (int)ldk);
+  const int kvalid = (int)(4 * (C1 + C2));
+  if (rc == EA_OK && ldk > kvalid)
+    rc = launch(patchify_pad_kernel, grid_1d(rows * (ldk - kvalid), 256), 256, 0, stream, "patchify_pad_kernel", (bf16*)a,
+                rows, kvalid, (int)ldk);
+  return rc;
+}
+
+extern "C" int ea_unpatchify(const void* y, void* out, int64_t B, int64_t C, int64_t F, int64_t H, int64_t W,
+                             int64_t ldy, void* stream) {
+  EA_REQUIRE(y && out, "ea_unpatchify: null pointer");
+  EA_REQUIRE(H % 2 == 0 && W % 2 == 0 && ldy >= 4 * C && ldy % 4 == 0, "ea_unpatchify: bad shape");
+  return launch(unpatchify_kernel, grid_1d(B * C * F * (H / 2) * (W / 2), 256), 256, 0, stream, "unpatchify_kernel",
+                (const bf16*)y, (bf16*)out, (int)B, (int)C, (int)F, (int)H, (int)W, (int)ldy);
+}
+
+extern "C" int ea_cfg_euler_step(const void* pred_uncond, const void* pred_text, const void* x, void* x_out, int64_t n,
+                                 float guidance_scale, int32_t use_cfg, float sigma, float sigma_next, void* stream) {
+  EA_REQUIRE(pred_uncond && x && x_out, "ea_cfg_euler_step: null pointer");
+  EA_REQUIRE(!use_cfg || pred_text, "ea_cfg_euler_step: CFG needs the text-conditioned prediction");
+  EA_REQUIRE(n > 0 && n % 2 == 0, "ea_cfg_euler_step: element count must be even");
+  const float dt = sigma_next - sigma;  // fp32 subtraction of fp32 sigmas, as the scheduler does
+  return launch(cfg_euler_kernel, grid_1d(n / 2, 256), 256, 0, stream, "cfg_euler_kernel", (const bf16*)pred_uncond,
+                (const bf16*)pred_text, (const bf16*)x, (bf16*)x_out, n, guidance_scale, use_cfg, dt);
+}
+
+extern "C" int ea_dequant_e4m3(const void* w8, void* w16, int64_t n, void* stream) {
   EA_REQUIRE(w8 && w16 && n > 0, "ea_dequant_e4m3: bad arguments");
   EA_REQUIRE((reinterpret_cast<uintptr_t>(w8) & 15) == 0 && (reinterpret_cast<uintptr_t>(w16) & 15) == 0,
              "ea_dequant_e4m3: pointers must be 16-byte aligned");
-  const int64_t threads = (n + 15) / 16;
-  ea::dequant_e4m3_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, stream>>>((const uint8_t*)w8, (ea::bf16*)w16, n);
-  ea::count_launch();
-  return ea::check_launch("dequant_e4m3_kernel");
+  return launch(dequant_e4m3_kernel, grid_1d((n + 15) / 16, 256), 256, 0, stream, "dequant_e4m3_kernel",
+                (const uint8_t*)w8, (bf16*)w16, n);
 }
 
-extern "C" int ea_l1_sums(const void* cur, const void* prev, void* sums, int64_t n, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+extern "C" int ea_l1_sums(const void* cur, const void* prev, void* sums, int64_t n, void* stream) {
   EA_REQUIRE(cur && prev && sums && n > 0 && n % 2 == 0, "ea_l1_sums: bad arguments");
-  cudaMemsetAsync(sums, 0, 2 * sizeof(double), stream);
-  int64_t blocks = (n / 2 + 255) / 256;
-  if (blocks > 4 * ea::sm_count()) blocks = 4 * ea::sm_count();
-  ea::l1_sums_kernel<<<(unsigned)blocks, 256, 0, stream>>>((const ea::bf16*)cur, (const ea::bf16*)prev, (double*)sums, n);
-  ea::count_launch();
-  return ea::check_launch("l1_sums_kernel");
+  const cudaError_t e = cudaMemsetAsync(sums, 0, 2 * sizeof(double), static_cast<cudaStream_t>(stream));
+  if (e != cudaSuccess) return fail(EA_ERR_CUDA, std::string("cudaMemsetAsync(l1_sums_kernel): ") + cudaGetErrorString(e));
+  const unsigned blocks = std::min(grid_1d(n / 2, 256), 4u * sm_count());
+  return launch(l1_sums_kernel, blocks, 256, 0, stream, "l1_sums_kernel", (const bf16*)cur, (const bf16*)prev,
+                (double*)sums, n);
 }
 
-extern "C" int ea_ew_addsub(const void* a, const void* b, void* out, int64_t n, int32_t subtract, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+extern "C" int ea_ew_addsub(const void* a, const void* b, void* out, int64_t n, int32_t subtract, void* stream) {
   EA_REQUIRE(a && b && out && n > 0 && n % 2 == 0, "ea_ew_addsub: bad arguments");
-  ea::ew_addsub_kernel<<<(unsigned)((n / 2 + 255) / 256), 256, 0, stream>>>((const ea::bf16*)a, (const ea::bf16*)b,
-                                                                           (ea::bf16*)out, n, subtract);
-  ea::count_launch();
-  return ea::check_launch("ew_addsub_kernel");
+  return launch(ew_addsub_kernel, grid_1d(n / 2, 256), 256, 0, stream, "ew_addsub_kernel", (const bf16*)a, (const bf16*)b,
+                (bf16*)out, n, subtract);
 }

@@ -239,8 +239,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
 // host launch
 // ------------------------------------------------------------------------------------------------
 template <int BN, int EPI>
-static int launch_gemm(const void* a, int64_t lda, const void* w, int64_t ldw, const GemmDevArgs& p,
-                       cudaStream_t stream) {
+static int launch_gemm(const void* a, int64_t lda, const void* w, int64_t ldw, const GemmDevArgs& p, void* stream) {
   CUtensorMap ta, tb;
   {
     uint64_t dims[2] = {(uint64_t)p.K, (uint64_t)p.M};
@@ -263,8 +262,7 @@ static int launch_gemm(const void* a, int64_t lda, const void* w, int64_t ldw, c
 }
 
 template <int EPI>
-static int dispatch_bn(const void* a, int64_t lda, const void* w, int64_t ldw, const GemmDevArgs& p,
-                       cudaStream_t stream) {
+static int dispatch_bn(const void* a, int64_t lda, const void* w, int64_t ldw, const GemmDevArgs& p, void* stream) {
   // Wide tiles unless they would leave most SMs idle.
   const int sms = sm_count();
   auto tiles = [&](int bn) { return (int64_t)((p.M + kTcBM - 1) / kTcBM) * ((p.N + bn - 1) / bn); };
@@ -278,8 +276,7 @@ static int dispatch_bn(const void* a, int64_t lda, const void* w, int64_t ldw, c
 
 using namespace ea;
 
-extern "C" int ea_gemm(const ea_gemm_args* g, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+extern "C" int ea_gemm(const ea_gemm_args* g, void* stream) {
   EA_REQUIRE(g != nullptr, "ea_gemm: null args");
   EA_REQUIRE(g->a && g->w && g->out, "ea_gemm: null pointer");
   EA_REQUIRE(g->M > 0 && g->N > 0 && g->K > 0, "ea_gemm: empty problem");
@@ -313,8 +310,7 @@ extern "C" int ea_gemm(const ea_gemm_args* g, void* stream_) {
   }
 }
 
-extern "C" int ea_qkv_gemm_ln_rope(const ea_qkv_args* g, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+extern "C" int ea_qkv_gemm_ln_rope(const ea_qkv_args* g, void* stream) {
   EA_REQUIRE(g != nullptr, "ea_qkv: null args");
   EA_REQUIRE(g->a && g->w && g->bias && ((g->q && g->k && g->v) || g->peers), "ea_qkv: null pointer");
   EA_REQUIRE(g->ln_q_w && g->ln_q_b && g->ln_k_w && g->ln_k_b, "ea_qkv: null LayerNorm parameter");

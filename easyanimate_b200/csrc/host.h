@@ -39,17 +39,27 @@ void count_launch();
 // Raises kern's dynamic shared-memory limit to `bytes` on the current device, once per device (`done` belongs to kern).
 int set_max_dynamic_smem(const void* kern, int bytes, PerDeviceFlag& done, const char* what);
 
-// Launches kern(args...) as a persistent grid of min(tiles, SMs) CTAs of `threads` with `smem_bytes` of dynamic shared
-// memory (set_max_dynamic_smem with `smem_done` first), counts the launch and reports a launch error.
-template <class... Args>
-int launch_persistent(void (*kern)(Args...), int64_t tiles, int threads, int smem_bytes, PerDeviceFlag& smem_done,
-                      cudaStream_t stream, const char* what, const Args&... args) {
-  const int rc = set_max_dynamic_smem(reinterpret_cast<const void*>(kern), smem_bytes, smem_done, what);
-  if (rc) return rc;
-  const int grid = (int)(tiles < sm_count() ? tiles : sm_count());
-  kern<<<grid, threads, smem_bytes, stream>>>(args...);
+// Blocks of `threads` needed to cover n work items.
+inline unsigned grid_1d(int64_t n, int threads) { return (unsigned)((n + threads - 1) / threads); }
+
+// Launches kern(args...) on `stream` (the C ABI's void* stream), counts the launch for ea_launch_count() and reports a
+// launch error under the name `what`. Every kernel launch of the library goes through here.
+template <class... Params, class... Args>
+int launch(void (*kern)(Params...), dim3 grid, dim3 block, size_t smem_bytes, void* stream, const char* what,
+           const Args&... args) {
+  kern<<<grid, block, smem_bytes, reinterpret_cast<cudaStream_t>(stream)>>>(args...);
   count_launch();
   return check_launch(what);
+}
+
+// launch() as a persistent grid of min(tiles, SMs) CTAs of `threads` with `smem_bytes` of dynamic shared memory
+// (set_max_dynamic_smem with `smem_done` first).
+template <class... Params, class... Args>
+int launch_persistent(void (*kern)(Params...), int64_t tiles, int threads, int smem_bytes, PerDeviceFlag& smem_done,
+                      void* stream, const char* what, const Args&... args) {
+  const int rc = set_max_dynamic_smem(reinterpret_cast<const void*>(kern), smem_bytes, smem_done, what);
+  if (rc) return rc;
+  return launch(kern, (unsigned)(tiles < sm_count() ? tiles : sm_count()), threads, smem_bytes, stream, what, args...);
 }
 
 }  // namespace ea

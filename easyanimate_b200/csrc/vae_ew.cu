@@ -9,8 +9,6 @@
 
 namespace ea {
 
-extern void count_launch();
-
 // z[b][c][t][h][w] (planar, C channels) -> y[t][h][w][Cpad] = bf16(W z + bias) for c < C, 0 above.
 // autoencoder_magvit.py:281 post_quant_conv (1x1x1 Conv3d) fused with the NCTHW -> THWC transposition.
 __global__ void vae_prepare_latents_kernel(const bf16* __restrict__ z, const bf16* __restrict__ w,
@@ -117,18 +115,21 @@ EA_DEVICE void gn_rows_sum(const double* __restrict__ part, int i, int G, int ro
     b += __shfl_xor_sync(0xffffffffu, b, off);
   }
 }
+// (mean, rstd) of group i from its fp64 (sum, sum of squares) over `count` elements
+EA_DEVICE void gn_store_stats(float* __restrict__ stats, int i, double a, double b, double count, float eps) {
+  const double mean = a / count;
+  double var = b / count - mean * mean;
+  var = var < 0 ? 0 : var;
+  stats[2 * i] = (float)mean;
+  stats[2 * i + 1] = (float)(1.0 / sqrt(var + (double)eps));
+}
 __global__ void gn_finalize_kernel(const double* __restrict__ part, float* __restrict__ stats, int n, int G, int rows,
                                    double count, float eps) {
   const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;  // (frame, group)
   if (i >= n) return;
   double a, b;
   gn_rows_sum(part, i, G, rows, a, b);
-  if ((threadIdx.x & 31) != 0) return;
-  const double mean = a / count;
-  double var = b / count - mean * mean;
-  var = var < 0 ? 0 : var;
-  stats[2 * i] = (float)mean;
-  stats[2 * i + 1] = (float)(1.0 / sqrt(var + (double)eps));
+  if ((threadIdx.x & 31) == 0) gn_store_stats(stats, i, a, b, count, eps);
 }
 // Strip-parallel decode: the rows of ONE rank reduced to a (sum, sum of squares) pair per (frame, group) ...
 __global__ void gn_sums_kernel(const double* __restrict__ part, double* __restrict__ sums, int n, int G, int rows) {
@@ -150,11 +151,7 @@ __global__ void gn_finalize_parts_kernel(const double* __restrict__ sums, float*
     a += sums[((int64_t)r * n + i) * 2];
     b += sums[((int64_t)r * n + i) * 2 + 1];
   }
-  const double mean = a / count;
-  double var = b / count - mean * mean;
-  var = var < 0 ? 0 : var;
-  stats[2 * i] = (float)mean;
-  stats[2 * i + 1] = (float)(1.0 / sqrt(var + (double)eps));
+  gn_store_stats(stats, i, a, b, count, eps);
 }
 // y = [silu](bf16((x - mean) * rstd * gamma + beta)); one 8-channel vector per thread
 __global__ void gn_apply_kernel(const bf16* __restrict__ x, bf16* __restrict__ y, const bf16* __restrict__ gamma,
@@ -278,7 +275,7 @@ __global__ void __launch_bounds__(256) softmax_rows_kernel(const float* __restri
   bf16* out = p + (int64_t)blockIdx.x * ldp;
   float mx = -INFINITY;
   for (int i = threadIdx.x; i < N; i += blockDim.x) mx = fmaxf(mx, row[i]);
-  for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  mx = warp_max(mx);
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = mx;
   __syncthreads();
   mx = red[0];
@@ -286,7 +283,7 @@ __global__ void __launch_bounds__(256) softmax_rows_kernel(const float* __restri
   __syncthreads();
   float sum = 0.f;
   for (int i = threadIdx.x; i < N; i += blockDim.x) sum += expf(row[i] - mx);
-  for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+  sum = warp_sum(sum);
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = sum;
   __syncthreads();
   sum = 0.f;
@@ -311,17 +308,24 @@ __global__ void transpose2d_kernel(const bf16* __restrict__ in, bf16* __restrict
   }
 }
 
+// idx -> (plane, row, col) of a planes x rows x cols index space, col fastest
+struct PlanarPos {
+  int pl, r, c;
+};
+EA_DEVICE PlanarPos planar_pos(int64_t idx, int rows, int cols) {
+  const int c = (int)(idx % cols);
+  const int r = (int)((idx / cols) % rows);
+  return {(int)(idx / ((int64_t)cols * rows)), r, c};
+}
+
 // dst[..., y0+i, x0+j] blended in place with src tile: dst = src*(1-wgt) + dst*wgt  (blend_v / blend_h,
 // autoencoder_magvit.py:319-337), planar [C*T][H][W] images. axis 0: ramp along rows, 1: along columns.
 __global__ void blend_kernel(const bf16* __restrict__ a, int64_t a_plane, int a_ld, int a_off_r, int a_off_c,
                              bf16* __restrict__ b, int64_t b_plane, int b_ld, int planes, int rows, int cols, int extent,
                              int axis) {
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const int64_t total = (int64_t)planes * rows * cols;
-  if (idx >= total) return;
-  const int c = (int)(idx % cols);
-  const int r = (int)((idx / cols) % rows);
-  const int pl = (int)(idx / ((int64_t)cols * rows));
+  if (idx >= (int64_t)planes * rows * cols) return;
+  const auto [pl, r, c] = planar_pos(idx, rows, cols);
   const int k = axis == 0 ? r : c;
   // python: b = a * (1 - k/extent) + b * (k/extent): python-float weights enter the bf16 ops at fp32 precision
   const float wb = (float)((double)k / (double)extent);
@@ -337,11 +341,8 @@ __global__ void blend_kernel(const bf16* __restrict__ a, int64_t a_plane, int a_
 __global__ void copy2d_kernel(const bf16* __restrict__ src, int64_t s_plane, int s_ld, bf16* __restrict__ dst,
                               int64_t d_plane, int d_ld, int planes, int rows, int cols) {
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const int64_t total = (int64_t)planes * rows * cols;
-  if (idx >= total) return;
-  const int c = (int)(idx % cols);
-  const int r = (int)((idx / cols) % rows);
-  const int pl = (int)(idx / ((int64_t)cols * rows));
+  if (idx >= (int64_t)planes * rows * cols) return;
+  const auto [pl, r, c] = planar_pos(idx, rows, cols);
   dst[pl * d_plane + (int64_t)r * d_ld + c] = src[pl * s_plane + (int64_t)r * s_ld + c];
 }
 
@@ -349,11 +350,8 @@ __global__ void copy2d_kernel(const bf16* __restrict__ src, int64_t s_plane, int
 __global__ void corner_blend_kernel(const bf16* __restrict__ src, bf16* __restrict__ dst, int64_t d_plane, int d_ld,
                                     int planes, int Hc, int Wc) {
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const int64_t total = (int64_t)planes * Hc * Wc;
-  if (idx >= total) return;
-  const int c = (int)(idx % Wc);
-  const int r = (int)((idx / Wc) % Hc);
-  const int pl = (int)(idx / ((int64_t)Wc * Hc));
+  if (idx >= (int64_t)planes * Hc * Wc) return;
+  const auto [pl, r, c] = planar_pos(idx, Hc, Wc);
   // torch.linspace(0,1,N) in fp32: i * (1/(N-1)) evaluated symmetric; fp32 weights * bf16 -> fp32 math, bf16 on store
   const float wx = Wc > 1 ? (float)c / (float)(Wc - 1) : 0.f;
   const float wy = Hc > 1 ? (float)r / (float)(Hc - 1) : 0.f;
@@ -373,14 +371,7 @@ __global__ void frames_out_kernel(const bf16* __restrict__ x, OutT* __restrict__
   if (i0 >= n) return;
   float v[8];
   if (i0 + 8 <= n) {
-    const uint4 u = *reinterpret_cast<const uint4*>(x + i0);
-    const uint32_t uw[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const float2 f = unpack_bf16x2(uw[k]);
-      v[2 * k] = f.x;
-      v[2 * k + 1] = f.y;
-    }
+    unpack_bf16x8(*reinterpret_cast<const uint4*>(x + i0), v);
   } else {
     for (int k = 0; k < 8; ++k) v[k] = i0 + k < n ? __bfloat162float(x[i0 + k]) : 0.f;
   }
@@ -418,33 +409,25 @@ __global__ void frames_out_kernel(const bf16* __restrict__ x, OutT* __restrict__
 
 using namespace ea;
 
-extern "C" int ea_frames_out(const void* x, void* out, int64_t n, int32_t out_kind, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+extern "C" int ea_frames_out(const void* x, void* out, int64_t n, int32_t out_kind, void* stream) {
   EA_REQUIRE(x && out && n > 0, "ea_frames_out: bad arguments");
   EA_REQUIRE(out_kind == EA_FRAMES_F32 || out_kind == EA_FRAMES_U8, "ea_frames_out: out_kind must be EA_FRAMES_F32 or EA_FRAMES_U8");
   EA_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0,
              "ea_frames_out: pointers must be 16-byte aligned");
-  const int64_t threads = (n + 7) / 8;
-  const unsigned blocks = (unsigned)((threads + 255) / 256);
+  const unsigned blocks = grid_1d((n + 7) / 8, 256);
   if (out_kind == EA_FRAMES_F32)
-    frames_out_kernel<float><<<blocks, 256, 0, stream>>>((const bf16*)x, (float*)out, n);
-  else
-    frames_out_kernel<uint8_t><<<blocks, 256, 0, stream>>>((const bf16*)x, (uint8_t*)out, n);
-  count_launch();
-  return check_launch("frames_out_kernel");
+    return launch(frames_out_kernel<float>, blocks, 256, 0, stream, "frames_out_kernel", (const bf16*)x, (float*)out, n);
+  return launch(frames_out_kernel<uint8_t>, blocks, 256, 0, stream, "frames_out_kernel", (const bf16*)x, (uint8_t*)out, n);
 }
 
 extern "C" int ea_vae_prepare_latents(const void* z, const void* w, const void* bias, void* y, int64_t C, int64_t Cpad,
-                                      int64_t T, int64_t H, int64_t W, float in_scale, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+                                      int64_t T, int64_t H, int64_t W, float in_scale, void* stream) {
   EA_REQUIRE(z && w && bias && y, "ea_vae_prepare_latents: null pointer");
   EA_REQUIRE(C > 0 && C <= 32 && Cpad >= C && Cpad % 8 == 0, "ea_vae_prepare_latents: need C <= 32, Cpad % 8 == 0");
   const int64_t thw = T * H * W;
   const size_t smem = (size_t)(C * C + C) * sizeof(float);
-  vae_prepare_latents_kernel<<<(unsigned)((thw + 127) / 128), 128, smem, stream>>>(
-      (const bf16*)z, (const bf16*)w, (const bf16*)bias, (bf16*)y, (int)C, (int)Cpad, thw, thw, in_scale);
-  count_launch();
-  return check_launch("vae_prepare_latents_kernel");
+  return launch(vae_prepare_latents_kernel, grid_1d(thw, 128), 128, smem, stream, "vae_prepare_latents_kernel",
+                (const bf16*)z, (const bf16*)w, (const bf16*)bias, (bf16*)y, (int)C, (int)Cpad, thw, thw, in_scale);
 }
 
 extern "C" size_t ea_groupnorm_workspace(int64_t frames, int64_t rows, int64_t groups) {
@@ -452,57 +435,48 @@ extern "C" size_t ea_groupnorm_workspace(int64_t frames, int64_t rows, int64_t g
 }
 
 static int gn_row_partials(const char* who, const void* x, void* workspace, size_t workspace_bytes, int64_t frames, int64_t rows,
-                           int64_t W, int64_t C, int64_t groups, cudaStream_t stream) {
+                           int64_t W, int64_t C, int64_t groups, void* stream) {
   if (!(C % 8 == 0 && C % groups == 0 && C <= 2048 && 256 % (C / 8) == 0))
     return fail(EA_ERR_INVALID, std::string(who) + ": C must be a multiple of 8 dividing into 256 threads, and of groups");
   if (workspace_bytes < ea_groupnorm_workspace(frames, rows, groups)) return fail(EA_ERR_WORKSPACE, std::string(who) + ": workspace too small");
   if (!(frames > 0 && rows > 0 && W > 0 && frames <= 65535 && rows < (1ll << 31) && W < (1ll << 24)))
     return fail(EA_ERR_INVALID, std::string(who) + ": bad frame / row / width count");
-  dim3 grid((unsigned)rows, (unsigned)frames);
   const size_t smem = 2 * (size_t)(256 / (C / 8)) * C * sizeof(float);  // 16 KB
-  gn_row_partial_kernel<<<grid, 256, smem, stream>>>((const bf16*)x, (double*)workspace, (int)rows, (int)W, (int)C, (int)groups);
-  count_launch();
-  return EA_OK;
+  return launch(gn_row_partial_kernel, dim3((unsigned)rows, (unsigned)frames), 256, smem, stream, "gn_row_partial_kernel",
+                (const bf16*)x, (double*)workspace, (int)rows, (int)W, (int)C, (int)groups);
 }
 
+// The reductions over the row partials take one warp per (frame, group), four per block.
 extern "C" int ea_groupnorm_stats(const void* x, void* stats, void* workspace, size_t workspace_bytes, int64_t frames,
-                                  int64_t rows, int64_t W, int64_t C, int64_t groups, float eps, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+                                  int64_t rows, int64_t W, int64_t C, int64_t groups, float eps, void* stream) {
   EA_REQUIRE(x && stats && workspace, "ea_groupnorm_stats: null pointer");
-  int rc = gn_row_partials("ea_groupnorm_stats", x, workspace, workspace_bytes, frames, rows, W, C, groups, stream);
+  const int rc = gn_row_partials("ea_groupnorm_stats", x, workspace, workspace_bytes, frames, rows, W, C, groups, stream);
   if (rc) return rc;
   const int n = (int)(frames * groups);
-  gn_finalize_kernel<<<(n * 32 + 127) / 128, 128, 0, stream>>>((const double*)workspace, (float*)stats, n, (int)groups, (int)rows,
-                                                                (double)rows * (double)W * (double)(C / groups), eps);
-  count_launch();
-  return check_launch("groupnorm_stats");
+  return launch(gn_finalize_kernel, grid_1d(n * 32, 128), 128, 0, stream, "gn_finalize_kernel", (const double*)workspace,
+                (float*)stats, n, (int)groups, (int)rows, (double)rows * (double)W * (double)(C / groups), eps);
 }
 
 extern "C" int ea_groupnorm_sums(const void* x, void* sums, void* workspace, size_t workspace_bytes, int64_t frames,
-                                 int64_t rows, int64_t W, int64_t C, int64_t groups, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+                                 int64_t rows, int64_t W, int64_t C, int64_t groups, void* stream) {
   EA_REQUIRE(x && sums && workspace, "ea_groupnorm_sums: null pointer");
-  int rc = gn_row_partials("ea_groupnorm_sums", x, workspace, workspace_bytes, frames, rows, W, C, groups, stream);
+  const int rc = gn_row_partials("ea_groupnorm_sums", x, workspace, workspace_bytes, frames, rows, W, C, groups, stream);
   if (rc) return rc;
   const int n = (int)(frames * groups);
-  gn_sums_kernel<<<(n * 32 + 127) / 128, 128, 0, stream>>>((const double*)workspace, (double*)sums, n, (int)groups, (int)rows);
-  count_launch();
-  return check_launch("groupnorm_sums");
+  return launch(gn_sums_kernel, grid_1d(n * 32, 128), 128, 0, stream, "gn_sums_kernel", (const double*)workspace,
+                (double*)sums, n, (int)groups, (int)rows);
 }
 
 extern "C" int ea_groupnorm_finalize(const void* sums, void* stats, int64_t parts, int64_t frames, int64_t groups, double count,
-                                     float eps, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+                                     float eps, void* stream) {
   EA_REQUIRE(sums && stats && parts > 0 && frames > 0 && groups > 0 && count > 0, "ea_groupnorm_finalize: bad arguments");
   const int n = (int)(frames * groups);
-  gn_finalize_parts_kernel<<<(n + 127) / 128, 128, 0, stream>>>((const double*)sums, (float*)stats, n, (int)parts, count, eps);
-  count_launch();
-  return check_launch("gn_finalize_parts_kernel");
+  return launch(gn_finalize_parts_kernel, grid_1d(n, 128), 128, 0, stream, "gn_finalize_parts_kernel",
+                (const double*)sums, (float*)stats, n, (int)parts, count, eps);
 }
 
 extern "C" int ea_groupnorm_apply(const void* x, void* y, const void* gamma, const void* beta, const void* stats,
-                                  int64_t frames, int64_t HW, int64_t C, int64_t groups, int32_t silu, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+                                  int64_t frames, int64_t HW, int64_t C, int64_t groups, int32_t silu, void* stream) {
   EA_REQUIRE(x && y && gamma && beta && stats, "ea_groupnorm_apply: null pointer");
   EA_REQUIRE(C % 8 == 0 && C % groups == 0, "ea_groupnorm_apply: bad channel count");
   static const bool legacy = getenv("EA_GN_LEGACY_APPLY") != nullptr;  // A/B: the first (one vector per thread) kernel
@@ -510,80 +484,52 @@ extern "C" int ea_groupnorm_apply(const void* x, void* y, const void* gamma, con
     // ~8 blocks per SM and frame-sized work items: 1 024 pixels per block, never fewer than one wave of blocks per call
     int pix_per_block = 1024;
     while (pix_per_block > 64 && frames * ((HW + pix_per_block - 1) / pix_per_block) < 4 * (int64_t)sm_count()) pix_per_block >>= 1;
-    dim3 grid((unsigned)((HW + pix_per_block - 1) / pix_per_block), (unsigned)frames);
-    gn_apply2_kernel<<<grid, 256, 0, stream>>>((const bf16*)x, (bf16*)y, (const bf16*)gamma, (const bf16*)beta,
-                                               (const float*)stats, HW, (int)C, (int)groups, pix_per_block, silu);
-    count_launch();
-    return check_launch("gn_apply2_kernel");
+    return launch(gn_apply2_kernel, dim3(grid_1d(HW, pix_per_block), (unsigned)frames), 256, 0, stream, "gn_apply2_kernel",
+                  (const bf16*)x, (bf16*)y, (const bf16*)gamma, (const bf16*)beta, (const float*)stats, HW, (int)C,
+                  (int)groups, pix_per_block, silu);
   }
   const int64_t total_vec = frames * HW * (C / 8);
-  gn_apply_kernel<<<(unsigned)((total_vec + 255) / 256), 256, 0, stream>>>((const bf16*)x, (bf16*)y, (const bf16*)gamma,
-                                                                          (const bf16*)beta, (const float*)stats, HW,
-                                                                          (int)C, (int)groups, total_vec, silu);
-  count_launch();
-  return check_launch("gn_apply_kernel");
+  return launch(gn_apply_kernel, grid_1d(total_vec, 256), 256, 0, stream, "gn_apply_kernel", (const bf16*)x, (bf16*)y,
+                (const bf16*)gamma, (const bf16*)beta, (const float*)stats, HW, (int)C, (int)groups, total_vec, silu);
 }
 
-extern "C" int ea_upsample2x(const void* x, void* y, int64_t T, int64_t H, int64_t W, int64_t C, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+extern "C" int ea_upsample2x(const void* x, void* y, int64_t T, int64_t H, int64_t W, int64_t C, void* stream) {
   EA_REQUIRE(x && y && C % 8 == 0, "ea_upsample2x: bad arguments");
-  const int64_t total = T * 2 * H * 2 * W * (C / 8);
-  upsample2x_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>((const bf16*)x, (bf16*)y, T, (int)H, (int)W,
-                                                                        (int)C);
-  count_launch();
-  return check_launch("upsample2x_kernel");
+  return launch(upsample2x_kernel, grid_1d(T * 2 * H * 2 * W * (C / 8), 256), 256, 0, stream, "upsample2x_kernel",
+                (const bf16*)x, (bf16*)y, T, (int)H, (int)W, (int)C);
 }
 
-extern "C" int ea_softmax_rows(const void* s, void* p, int64_t M, int64_t N, int64_t lds, int64_t ldp, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+extern "C" int ea_softmax_rows(const void* s, void* p, int64_t M, int64_t N, int64_t lds, int64_t ldp, void* stream) {
   EA_REQUIRE(s && p && M > 0 && N > 0 && lds >= N && ldp >= N, "ea_softmax_rows: bad arguments");
-  softmax_rows_kernel<<<(unsigned)M, 256, 0, stream>>>((const float*)s, (bf16*)p, (int)N, lds, ldp);
-  count_launch();
-  return check_launch("softmax_rows_kernel");
+  return launch(softmax_rows_kernel, (unsigned)M, 256, 0, stream, "softmax_rows_kernel", (const float*)s, (bf16*)p, (int)N,
+                lds, ldp);
 }
 
-extern "C" int ea_transpose2d(const void* in, void* out, int64_t R, int64_t Cc, int64_t ldi, int64_t ldo,
-                              void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+extern "C" int ea_transpose2d(const void* in, void* out, int64_t R, int64_t Cc, int64_t ldi, int64_t ldo, void* stream) {
   EA_REQUIRE(in && out && R > 0 && Cc > 0 && ldi >= Cc && ldo >= R, "ea_transpose2d: bad arguments");
-  dim3 grid((unsigned)((Cc + 31) / 32), (unsigned)((R + 31) / 32));
-  transpose2d_kernel<<<grid, dim3(32, 8), 0, stream>>>((const bf16*)in, (bf16*)out, (int)R, (int)Cc, ldi, ldo);
-  count_launch();
-  return check_launch("transpose2d_kernel");
+  return launch(transpose2d_kernel, dim3(grid_1d(Cc, 32), grid_1d(R, 32)), dim3(32, 8), 0, stream, "transpose2d_kernel",
+                (const bf16*)in, (bf16*)out, (int)R, (int)Cc, ldi, ldo);
 }
 
 extern "C" int ea_tile_blend(const void* a, int64_t a_plane, int64_t a_ld, int64_t a_off_r, int64_t a_off_c, void* b,
                              int64_t b_plane, int64_t b_ld, int64_t planes, int64_t rows, int64_t cols, int64_t extent,
-                             int32_t axis, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+                             int32_t axis, void* stream) {
   EA_REQUIRE(a && b && planes > 0 && rows > 0 && cols > 0 && extent > 0, "ea_tile_blend: bad arguments");
-  const int64_t total = planes * rows * cols;
-  blend_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>((const bf16*)a, a_plane, (int)a_ld, (int)a_off_r,
-                                                                   (int)a_off_c, (bf16*)b, b_plane, (int)b_ld,
-                                                                   (int)planes, (int)rows, (int)cols, (int)extent, axis);
-  count_launch();
-  return check_launch("blend_kernel");
+  return launch(blend_kernel, grid_1d(planes * rows * cols, 256), 256, 0, stream, "blend_kernel", (const bf16*)a, a_plane,
+                (int)a_ld, (int)a_off_r, (int)a_off_c, (bf16*)b, b_plane, (int)b_ld, (int)planes, (int)rows, (int)cols,
+                (int)extent, axis);
 }
 
 extern "C" int ea_copy2d(const void* src, int64_t s_plane, int64_t s_ld, void* dst, int64_t d_plane, int64_t d_ld,
-                         int64_t planes, int64_t rows, int64_t cols, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+                         int64_t planes, int64_t rows, int64_t cols, void* stream) {
   EA_REQUIRE(src && dst && planes > 0 && rows > 0 && cols > 0, "ea_copy2d: bad arguments");
-  const int64_t total = planes * rows * cols;
-  copy2d_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>((const bf16*)src, s_plane, (int)s_ld, (bf16*)dst,
-                                                                    d_plane, (int)d_ld, (int)planes, (int)rows,
-                                                                    (int)cols);
-  count_launch();
-  return check_launch("copy2d_kernel");
+  return launch(copy2d_kernel, grid_1d(planes * rows * cols, 256), 256, 0, stream, "copy2d_kernel", (const bf16*)src,
+                s_plane, (int)s_ld, (bf16*)dst, d_plane, (int)d_ld, (int)planes, (int)rows, (int)cols);
 }
 
 extern "C" int ea_corner_blend(const void* src, void* dst, int64_t d_plane, int64_t d_ld, int64_t planes, int64_t Hc,
-                               int64_t Wc, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+                               int64_t Wc, void* stream) {
   EA_REQUIRE(src && dst && planes > 0 && Hc > 0 && Wc > 0, "ea_corner_blend: bad arguments");
-  const int64_t total = planes * Hc * Wc;
-  corner_blend_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>((const bf16*)src, (bf16*)dst, d_plane,
-                                                                          (int)d_ld, (int)planes, (int)Hc, (int)Wc);
-  count_launch();
-  return check_launch("corner_blend_kernel");
+  return launch(corner_blend_kernel, grid_1d(planes * Hc * Wc, 256), 256, 0, stream, "corner_blend_kernel",
+                (const bf16*)src, (bf16*)dst, d_plane, (int)d_ld, (int)planes, (int)Hc, (int)Wc);
 }

@@ -5,6 +5,7 @@ importing this package requires the in-tree CUDA library ``libea_b200.so`` (ther
 """
 from . import _lib  # noqa: F401  (fails loudly if the CUDA extension has not been built)
 from .autoencoder_magvit import AutoencoderKLMagvit
+from .long_video import generate_long_video
 from .pipeline import EasyAnimateSampler, rope_table
 from .pipelines import (EasyAnimateControlPipeline, EasyAnimateInpaintPipeline, EasyAnimatePipeline,
                         EasyAnimatePipelineOutput, load_pipeline)
@@ -16,4 +17,4 @@ name_to_autoencoder_magvit = {"AutoencoderKLMagvit": AutoencoderKLMagvit}
 
 __all__ = ["AutoencoderKLMagvit", "EasyAnimateControlPipeline", "EasyAnimateInpaintPipeline", "EasyAnimatePipeline",
            "EasyAnimatePipelineOutput", "EasyAnimateSampler", "EasyAnimateTransformer3DModel", "FlowMatchEulerDiscreteScheduler",
-           "load_pipeline", "name_to_autoencoder_magvit", "name_to_transformer3d", "rope_table"]
+           "generate_long_video", "load_pipeline", "name_to_autoencoder_magvit", "name_to_transformer3d", "rope_table"]

@@ -141,6 +141,7 @@ ea_ipc_close = _sig("ea_ipc_close", [vp])
 ea_conv3d_causal = _sig("ea_conv3d_causal", [C.POINTER(ConvArgs), vp])
 ea_vae_prepare_latents = _sig("ea_vae_prepare_latents", [vp, vp, vp, vp, i64, i64, i64, i64, i64, f32, vp])
 ea_frames_out = _sig("ea_frames_out", [vp, vp, i64, i32, vp])
+ea_frames_out_blend = _sig("ea_frames_out_blend", [vp, vp, i64, i64, i64, i64, i32, vp])
 ea_groupnorm_workspace = _sig("ea_groupnorm_workspace", [i64, i64, i64], C.c_size_t)
 ea_groupnorm_stats = _sig("ea_groupnorm_stats", [vp, vp, vp, C.c_size_t, i64, i64, i64, i64, i64, f32, vp])
 ea_groupnorm_sums = _sig("ea_groupnorm_sums", [vp, vp, vp, C.c_size_t, i64, i64, i64, i64, i64, vp])

@@ -489,11 +489,7 @@ class AutoencoderKLMagvit(nn.Module, ConfigMixinLite):
         utils.py:57 makes of the frames) is ONE kernel whose destination is `out`: a CUDA tensor, or with to_host=True a
         pinned host tensor the kernel writes over PCIe directly (no bf16 staging copy, no host-side .float()).  The call
         returns after the stream has been synchronised when the destination is on the host."""
-        self._latent_in_scale = 1.0 / float(self.config.scaling_factor)
-        try:
-            video = self._decode(latents)
-        finally:
-            self._latent_in_scale = 1.0
+        video = self.decode_scaled_video(latents)
         if out is None:
             out = (torch.empty(video.shape, dtype=dtype, pin_memory=True) if to_host
                    else torch.empty(video.shape, dtype=dtype, device=video.device))
@@ -501,6 +497,16 @@ class AutoencoderKLMagvit(nn.Module, ConfigMixinLite):
         if not out.is_cuda:
             torch.cuda.current_stream(video.device).synchronize()
         return out
+
+    @torch.no_grad()
+    def decode_scaled_video(self, latents: torch.Tensor) -> torch.Tensor:
+        """decode_scaled before its output tail: the decoded bf16 video [B,3,F,H,W] on the device, for callers that apply
+        a tail of their own (the long-video cross-fade, `vae_ops.frames_out_blend`)."""
+        self._latent_in_scale = 1.0 / float(self.config.scaling_factor)
+        try:
+            return self._decode(latents)
+        finally:
+            self._latent_in_scale = 1.0
 
     # ---- encode (I2V / inpaint conditioning prep) ---------------------------------------------------------------
     def _encode_one(self, x: torch.Tensor) -> torch.Tensor:

@@ -362,8 +362,17 @@ __global__ void corner_blend_kernel(const bf16* __restrict__ src, bf16* __restri
   *dp = __float2bfloat16_rn(wgt * s + (1.0f - wgt) * d);
 }
 
-// decode_latents' tail (pipeline_easyanimate.py:729,738-740): clamp(-1,1) -> /2 + 0.5 (two bf16 ops) -> clamp(0,1) ->
-// float32 (what `.cpu().float().numpy()` yields) or uint8 = trunc(255 * v) (utils.py:57 `(x * 255).numpy().astype(np.uint8)`).
+// decode_latents' tail (pipeline_easyanimate.py:729,738-740) on one decoded value: clamp(-1,1) -> /2 + 0.5 (two bf16 ops)
+// -> clamp(0,1), as float32 (what `.cpu().float().numpy()` yields).
+__device__ __forceinline__ float frame_value(float v) {
+  float a = fminf(fmaxf(v, -1.0f), 1.0f);     // video.clamp(-1, 1)      (NaN propagates like torch.clamp)
+  a = v != v ? v : a;
+  a = bf16_round(bf16_round(a * 0.5f) + 0.5f);  // video / 2 + 0.5        (bf16 tensor ops)
+  const float c = fminf(fmaxf(a, 0.0f), 1.0f);  // .clamp(0, 1)
+  return a != a ? a : c;
+}
+
+// frame_value as float32 or uint8 = trunc(255 * v) (utils.py:57 `(x * 255).numpy().astype(np.uint8)`).
 // `out` may be device memory or device-mapped pinned host memory: 8 elements per thread, 32 B (16 B) contiguous stores.
 template <typename OutT>
 __global__ void frames_out_kernel(const bf16* __restrict__ x, OutT* __restrict__ out, int64_t n) {
@@ -376,13 +385,7 @@ __global__ void frames_out_kernel(const bf16* __restrict__ x, OutT* __restrict__
     for (int k = 0; k < 8; ++k) v[k] = i0 + k < n ? __bfloat162float(x[i0 + k]) : 0.f;
   }
 #pragma unroll
-  for (int k = 0; k < 8; ++k) {
-    float a = fminf(fmaxf(v[k], -1.0f), 1.0f);   // video.clamp(-1, 1)      (NaN propagates like torch.clamp)
-    a = v[k] != v[k] ? v[k] : a;
-    a = bf16_round(bf16_round(a * 0.5f) + 0.5f);  // video / 2 + 0.5        (bf16 tensor ops)
-    const float c = fminf(fmaxf(a, 0.0f), 1.0f);  // .clamp(0, 1)
-    v[k] = a != a ? a : c;
-  }
+  for (int k = 0; k < 8; ++k) v[k] = frame_value(v[k]);
   if constexpr (sizeof(OutT) == 4) {
     if (i0 + 8 <= n) {
       *reinterpret_cast<float4*>(out + i0) = make_float4(v[0], v[1], v[2], v[3]);
@@ -405,6 +408,26 @@ __global__ void frames_out_kernel(const bf16* __restrict__ x, OutT* __restrict__
   }
 }
 
+// The long-video cross-fade (ui.py:524-531) fused with frames_out: x [planes, frames, frame_elems] bf16 is one decoded
+// window; frame t of plane p goes to dst + p * dst_plane + t * frame_elems.  The first `ov` frames are blended into what dst
+// holds, dst = dst * (1 - r_t) + f * r_t with r_t = float32(t / ov), every product and sum rounded on its own like torch's
+// float32 tensor ops (the _rn intrinsics keep nvcc from contracting them into an FMA); the other frames are stored as they are.
+// One row (plane, frame) per blockIdx.y.
+__global__ void frames_out_blend_kernel(const bf16* __restrict__ x, float* dst, int64_t frames, int64_t frame_elems,
+                                        int64_t dst_plane, int ov) {
+  const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= frame_elems) return;
+  const int64_t row = blockIdx.y, p = row / frames, t = row % frames;
+  const float f = frame_value(__bfloat162float(x[row * frame_elems + e]));
+  float* d = dst + p * dst_plane + t * frame_elems + e;
+  if (t < ov) {
+    const float r = (float)((double)t / (double)ov);  // np.float32(float(t) / float(ov))
+    *d = __fadd_rn(__fmul_rn(*d, __fsub_rn(1.0f, r)), __fmul_rn(f, r));
+  } else {
+    *d = f;
+  }
+}
+
 }  // namespace ea
 
 using namespace ea;
@@ -418,6 +441,17 @@ extern "C" int ea_frames_out(const void* x, void* out, int64_t n, int32_t out_ki
   if (out_kind == EA_FRAMES_F32)
     return launch(frames_out_kernel<float>, blocks, 256, 0, stream, "frames_out_kernel", (const bf16*)x, (float*)out, n);
   return launch(frames_out_kernel<uint8_t>, blocks, 256, 0, stream, "frames_out_kernel", (const bf16*)x, (uint8_t*)out, n);
+}
+
+extern "C" int ea_frames_out_blend(const void* x, void* dst, int64_t planes, int64_t frames, int64_t frame_elems,
+                                   int64_t dst_plane, int32_t ov, void* stream) {
+  EA_REQUIRE(x && dst && planes > 0 && frames > 0 && frame_elems > 0, "ea_frames_out_blend: bad arguments");
+  EA_REQUIRE(planes * frames <= 65535, "ea_frames_out_blend: planes * frames must be <= 65535");
+  EA_REQUIRE(ov >= 0 && ov <= frames, "ea_frames_out_blend: need 0 <= ov <= frames");
+  EA_REQUIRE(dst_plane >= frames * frame_elems, "ea_frames_out_blend: dst_plane must hold the window's frames");
+  const dim3 grid(grid_1d(frame_elems, 256), (unsigned)(planes * frames));
+  return launch(frames_out_blend_kernel, grid, 256, 0, stream, "frames_out_blend_kernel", (const bf16*)x, (float*)dst, frames,
+                frame_elems, dst_plane, (int)ov);
 }
 
 extern "C" int ea_vae_prepare_latents(const void* z, const void* w, const void* bias, void* y, int64_t C, int64_t Cpad,

@@ -432,6 +432,33 @@ class EasyAnimateInpaintPipeline(_NativePipelineBase):
                  crops_coords_top_left: Tuple[int, int] = (0, 0), clip_image=None, clip_apply_ratio: float = 0.40,
                  strength: float = 1.0, noise_aug_strength: float = 0.0563, comfyui_progressbar: bool = False,
                  timesteps: Optional[List[int]] = None):
+        args = {k: v for k, v in locals().items() if k not in ("self", "output_type", "return_dict")}
+        return self._finish(self.denoise_to_latents(**args), output_type, return_dict)
+
+    @torch.no_grad()
+    def denoise_to_latents(self, prompt: Union[str, List[str]] = None, video_length: Optional[int] = None,
+                           video: Optional[torch.Tensor] = None, mask_video: Optional[torch.Tensor] = None,
+                           masked_video_latents: Optional[torch.Tensor] = None, height: Optional[int] = None,
+                           width: Optional[int] = None, num_inference_steps: Optional[int] = 50,
+                           guidance_scale: Optional[float] = 5.0, negative_prompt: Optional[Union[str, List[str]]] = None,
+                           num_images_per_prompt: Optional[int] = 1, eta: Optional[float] = 0.0, generator=None,
+                           latents: Optional[torch.Tensor] = None, prompt_embeds: Optional[torch.Tensor] = None,
+                           prompt_embeds_2: Optional[torch.Tensor] = None,
+                           negative_prompt_embeds: Optional[torch.Tensor] = None,
+                           negative_prompt_embeds_2: Optional[torch.Tensor] = None,
+                           prompt_attention_mask: Optional[torch.Tensor] = None,
+                           prompt_attention_mask_2: Optional[torch.Tensor] = None,
+                           negative_prompt_attention_mask: Optional[torch.Tensor] = None,
+                           negative_prompt_attention_mask_2: Optional[torch.Tensor] = None,
+                           callback_on_step_end: Optional[Callable[..., Dict]] = None,
+                           callback_on_step_end_tensor_inputs: List[str] = ["latents"], guidance_rescale: float = 0.0,
+                           original_size: Optional[Tuple[int, int]] = (1024, 1024),
+                           target_size: Optional[Tuple[int, int]] = None, crops_coords_top_left: Tuple[int, int] = (0, 0),
+                           clip_image=None, clip_apply_ratio: float = 0.40, strength: float = 1.0,
+                           noise_aug_strength: float = 0.0563, comfyui_progressbar: bool = False,
+                           timesteps: Optional[List[int]] = None):
+        """`__call__` up to its final latents [B,16,F',h,w] bf16 on the device, without the decode: for callers that decode
+        with a tail of their own (generate_long_video).  Same arguments as `__call__` but `output_type` / `return_dict`."""
         height, width = self._prologue(prompt, height, width, guidance_scale, guidance_rescale, comfyui_progressbar, dict(
             negative_prompt=negative_prompt, prompt_embeds=prompt_embeds, negative_prompt_embeds=negative_prompt_embeds,
             prompt_attention_mask=prompt_attention_mask, negative_prompt_attention_mask=negative_prompt_attention_mask,
@@ -474,7 +501,7 @@ class EasyAnimateInpaintPipeline(_NativePipelineBase):
                              "Please verify the config of `pipeline.transformer` or your `mask_image` or `image` input.")
         latents = self._denoise(latents, pe, ne, height, width, first, steps, guidance_scale, inpaint_latents=inpaint,
                                 callback_on_step_end=callback_on_step_end, callback_tensor_inputs=callback_on_step_end_tensor_inputs)
-        return self._finish(latents, output_type, return_dict)
+        return latents
 
 
 class EasyAnimateControlPipeline(_NativePipelineBase):

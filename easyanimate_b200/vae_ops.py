@@ -78,6 +78,25 @@ def frames_out(video: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
     return out
 
 
+def frames_out_blend(video: torch.Tensor, out: torch.Tensor, overlap: int) -> torch.Tensor:
+    """frames_out (float32) of one decoded window video [B,C,F,H,W] into `out`, its slice [:, :, t0:t0+F] of the whole video,
+    cross-faded over the first `overlap` frames (ui.py:524-531): out = out * (1 - r) + frames * r, r = float32(t / overlap).
+    `out` is a CUDA tensor or a PINNED host tensor, like frames_out's."""
+    _req(video, name="video")
+    assert video.dim() == 5 and video.is_contiguous() and out.shape == video.shape, (video.shape, out.shape)
+    if out.dtype != torch.float32:
+        raise L.EaError(f"frames_out_blend writes float32, got {out.dtype}")
+    if not out.is_cuda and not out.is_pinned():
+        raise L.EaError("frames_out_blend: a host destination must be pinned memory (torch.empty(..., pin_memory=True))")
+    B, Cc, F, H, W = video.shape
+    plane = out.stride(1)
+    if out.stride(4) != 1 or out.stride(3) != W or out.stride(2) != H * W or out.stride(0) != Cc * plane:
+        raise L.EaError(f"frames_out_blend: `out` must be a frame range of a contiguous video, got strides {out.stride()}")
+    L.check(L.ea_frames_out_blend(_p(video), out.data_ptr(), B * Cc, F, H * W, plane, int(overlap), _stream()),
+            "ea_frames_out_blend")
+    return out
+
+
 def groupnorm(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, groups: int, eps: float, silu: bool) -> torch.Tensor:
     """Per-frame GroupNorm (+SiLU) of x [T,H,W,C]."""
     _req(x, name="x")

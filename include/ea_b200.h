@@ -290,6 +290,14 @@ int ea_vae_prepare_latents(const void* z, const void* w, const void* bias, void*
 enum { EA_FRAMES_F32 = 0, EA_FRAMES_U8 = 1 };
 int ea_frames_out(const void* x, void* out, int64_t n, int32_t out_kind, void* stream);
 
+/* ea_frames_out (float32) fused with the long-video cross-fade (ui.py:524-531): x [planes, frames, frame_elems] bf16 is one
+ * decoded window, and its frame t of plane p goes to dst + p * dst_plane + t * frame_elems (float32; the window's slice of
+ * the whole video, a device pointer or a device-mapped pinned host pointer).  For t < ov, dst = dst * (1 - r) + f * r with
+ * r = float32(t / ov), each product and sum rounded on its own like torch's float32 tensor ops; the other frames are
+ * overwritten with f.  ov = 0 is a plain strided ea_frames_out.  planes * frames <= 65535, 0 <= ov <= frames. */
+int ea_frames_out_blend(const void* x, void* dst, int64_t planes, int64_t frames, int64_t frame_elems, int64_t dst_plane,
+                        int32_t ov, void* stream);
+
 /* Per-frame GroupNorm (common.py:301-319 with set_3dgroupnorm; omnigen_enc_dec.py:603-609) of x [frames, rows, W, C]:
  * stats[frames,groups,2] = (mean, rstd) fp32; workspace = ea_groupnorm_workspace() bytes of scratch.  The statistics are
  * accumulated per image row and the rows added in fp64, so they do not depend on how a frame's rows are split over GPUs. */

@@ -193,23 +193,10 @@ def cfg_euler_step(noise_pred: torch.Tensor, latents: torch.Tensor, guidance_sca
     return out
 
 
-def rel_l1_distance(cur: torch.Tensor, prev: torch.Tensor) -> float:
-    """TeaCache.compute_rel_l1_distance (transformer3d.py:113-117): (|cur-prev|.mean() / |prev|.mean()).item() with the
-    reference's bf16 rounding of each intermediate.  Synchronises the stream (the reference's .cpu().item() does too)."""
-    _req(cur, name="cur"); _req(prev, name="prev")
-    assert cur.shape == prev.shape and cur.is_contiguous() and prev.is_contiguous()
-    sums = torch.empty((2,), device=cur.device, dtype=torch.float64)
-    L.check(L.ea_l1_sums(_p(cur), _p(prev), _p(sums), cur.numel(), _stream()), "ea_l1_sums")
-    num, den = (float(x) for x in sums.cpu())
-    n = cur.numel()
-    mean_diff = torch.tensor(num / n, dtype=torch.float32).to(bf16)  # .mean() of a bf16 tensor is a bf16 scalar
-    mean_prev = torch.tensor(den / n, dtype=torch.float32).to(bf16)
-    return float((mean_diff / mean_prev).item())
-
-
 def l1_sums(cur: torch.Tensor, prev: torch.Tensor) -> Tuple[float, float]:
-    """(sum |bf16(cur - prev)|, sum |prev|) as the two doubles ea_l1_sums produces: the additive pieces of
-    rel_l1_distance, for callers that combine them across ranks first (sequence parallelism)."""
+    """(sum |bf16(cur - prev)|, sum |prev|) as the two doubles ea_l1_sums produces: the additive pieces of TeaCache's
+    rel-L1 distance, which callers may sum over ranks before rel_l1_from_sums.  Synchronises the stream (the reference's
+    .cpu().item() does too)."""
     _req(cur, name="cur"); _req(prev, name="prev")
     assert cur.shape == prev.shape and cur.is_contiguous() and prev.is_contiguous()
     sums = torch.empty((2,), device=cur.device, dtype=torch.float64)
@@ -219,8 +206,9 @@ def l1_sums(cur: torch.Tensor, prev: torch.Tensor) -> Tuple[float, float]:
 
 
 def rel_l1_from_sums(num: float, den: float, n: int) -> float:
-    """The reference's bf16 rounding of each mean and of their ratio (transformer3d.py:113-117) from global sums."""
-    mean_diff = torch.tensor(num / n, dtype=torch.float32).to(bf16)
+    """TeaCache.compute_rel_l1_distance (transformer3d.py:113-117), (|cur-prev|.mean() / |prev|.mean()).item(), from the
+    sums of l1_sums over n elements, with the reference's bf16 rounding of each mean and of their ratio."""
+    mean_diff = torch.tensor(num / n, dtype=torch.float32).to(bf16)  # .mean() of a bf16 tensor is a bf16 scalar
     mean_prev = torch.tensor(den / n, dtype=torch.float32).to(bf16)
     return float((mean_diff / mean_prev).item())
 

@@ -193,9 +193,6 @@ class UlyssesAttention:
         dist.all_gather_into_tensor(out, x_loc.contiguous(), group=self.group)
         return out.view(self.world, B, S_loc, c).permute(1, 0, 2, 3).reshape(B * self.world * S_loc, c).contiguous()
 
-    def all_reduce_sums(self, values) -> list:
-        return all_reduce_floats(values, self.group)
-
     # ---- attention with the two exchanges -----------------------------------------------------------------------
     def attention(self, q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, S_t: int):
         """q, k, v [B, H, S_t + S_loc, 64]: ALL heads, the replicated text rows first, then this rank's video tokens.

@@ -563,19 +563,16 @@ class EasyAnimateTransformer3DModel(nn.Module, ConfigMixinLite):
             if tc.cnt == 0 or tc.cnt == tc.num_steps - 1:
                 tc.accumulated_rel_l1_distance = 0
             else:
+                # the decision must be the reference's (one per step, from the means over ALL tokens of BOTH CFG branches)
+                # and the same on every rank: the additive pieces are summed over the ranks of this video (none on one GPU)
+                from .sequence_parallel import all_reduce_floats, group_size
                 groups = [g for g in ((sp.group if sp is not None else None), self.cfg_parallel_group) if g is not None]
-                if not groups:
-                    dist = ops.rel_l1_distance(modulated, tc.previous_modulated_input)
-                else:
-                    # the decision must be the reference's (one per step, from the means over ALL tokens of BOTH CFG
-                    # branches) and the same on every rank: combine the additive pieces over the ranks of this video
-                    from .sequence_parallel import all_reduce_floats, group_size
-                    num, den = ops.l1_sums(modulated, tc.previous_modulated_input)
-                    n = modulated.numel()
-                    for g in groups:
-                        num, den = all_reduce_floats((num, den), g)
-                        n *= group_size(g)
-                    dist = ops.rel_l1_from_sums(num, den, n)
+                num, den = ops.l1_sums(modulated, tc.previous_modulated_input)
+                n = modulated.numel()
+                for g in groups:
+                    num, den = all_reduce_floats((num, den), g)
+                    n *= group_size(g)
+                dist = ops.rel_l1_from_sums(num, den, n)
                 tc.accumulated_rel_l1_distance += tc.rescale_func(dist)
                 if tc.accumulated_rel_l1_distance < tc.rel_l1_thresh:
                     should_calc = False

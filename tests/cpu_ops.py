@@ -1,8 +1,9 @@
 """Torch (CPU) stand-ins for the entry points of easyanimate_b200.ops that EasyAnimateTransformer3DModel.forward calls, with
 the argument conventions of the real wrappers (shapes, in-place outputs, row-per-batch gates, head-major q/k/v, patchify
-column order) and the rounding points documented in include/ea_b200.h.  TEST INFRASTRUCTURE: they let the CPU suite run the
-product module's HOST LOGIC (buffer plumbing, stream split, sequence-parallel sharding) end to end without a GPU; they are
-never used by the product path."""
+column order) and the rounding points documented in include/ea_b200.h, and for those of easyanimate_b200.vae_ops.
+TEST INFRASTRUCTURE: `use_stand_ins` installs them all, so that the CPU suite runs the product modules' HOST LOGIC (buffer
+plumbing, stream split, sequence-parallel sharding, decode dispatch) end to end without a GPU; they are never used by the
+product path."""
 import math
 
 import torch
@@ -139,20 +140,6 @@ def l1_sums(cur, prev):
     return num, prev.double().abs().sum().item()
 
 
-def rel_l1_distance(cur, prev):
-    from easyanimate_b200.ops import rel_l1_from_sums
-    num, den = l1_sums(cur, prev)
-    return rel_l1_from_sums(num, den, cur.numel())
-
-
-def install(monkeypatch):
-    """Route easyanimate_b200.ops (as seen by transformer3d) to the stand-ins above."""
-    from easyanimate_b200 import ops
-    for name in ("gemm", "skinny_linear", "layernorm_modulate", "rmsnorm", "timestep_embedding", "patchify", "unpatchify",
-                 "qkv_gemm_ln_rope", "attention", "ew_add", "rel_l1_distance", "l1_sums"):
-        monkeypatch.setattr(ops, name, globals()[name])
-
-
 # -----------------------------------------------------------------------------------------------------------------------
 # VAE entry points (easyanimate_b200.vae_ops): channels-last [T,H,W,C] activations for one batch element
 # -----------------------------------------------------------------------------------------------------------------------
@@ -275,17 +262,14 @@ def frames_out(video, out):
     return out
 
 
-def install_fp8(monkeypatch):
-    from easyanimate_b200 import ops
-    monkeypatch.setattr(ops, "dequant_e4m3", dequant_e4m3)
-
-
-def install_vae(monkeypatch):
-    from easyanimate_b200 import ops, vae_ops
-    for name in ("conv3d_causal", "prepare_latents", "groupnorm", "groupnorm_sums", "groupnorm_from_sums", "upsample2x",
-                 "spatial_attention", "tile_blend", "copy2d", "corner_blend", "frames_out"):
-        monkeypatch.setattr(vae_ops, name, globals()[name])
-    monkeypatch.setattr(ops, "gemm", gemm)
+def frames_out_blend(video, out, overlap):
+    """ea_frames_out_blend as the reference's tensor ops (pipeline_easyanimate.py:738-741, then ui.py:524-531)."""
+    f = (video.clamp(-1, 1) / 2 + 0.5).clamp(0, 1).float()
+    if overlap:
+        r = torch.tensor([float(i) / float(overlap) for i in range(overlap)], dtype=torch.float32).view(1, 1, -1, 1, 1)
+        out[:, :, :overlap] = out[:, :, :overlap] * (1 - r) + f[:, :, :overlap] * r
+    out[:, :, overlap:] = f[:, :, overlap:]
+    return out
 
 
 def cfg_euler_step(noise_pred, latents, guidance_scale, sigma, sigma_next, use_cfg=True):
@@ -297,3 +281,31 @@ def cfg_euler_step(noise_pred, latents, guidance_scale, sigma, sigma_next, use_c
         v = noise_pred
     dt = torch.tensor(sigma_next - sigma, dtype=torch.float32).to(bf16)
     return (latents.float() + (dt * v).float()).to(bf16)
+
+
+OPS = ("gemm", "skinny_linear", "layernorm_modulate", "rmsnorm", "timestep_embedding", "patchify", "unpatchify", "qkv_gemm_ln_rope",
+       "attention", "ew_add", "l1_sums", "cfg_euler_step", "dequant_e4m3")
+VAE_OPS = ("conv3d_causal", "prepare_latents", "groupnorm", "groupnorm_sums", "groupnorm_from_sums", "upsample2x",
+           "spatial_attention", "tile_blend", "copy2d", "corner_blend", "frames_out", "frames_out_blend")
+
+
+def _decode_scaled(self, latents, out=None, dtype=torch.float32, to_host=False):
+    """AutoencoderKLMagvit.decode_scaled with its tail in host memory (pinned buffers and stream synchronisation need a GPU)."""
+    video = self.decode_scaled_video(latents)
+    return frames_out(video.contiguous(), torch.empty(video.shape, dtype=dtype) if out is None else out)
+
+
+def use_stand_ins(mp, **fakes):
+    """Run the product's host logic on the CPU: every entry point of easyanimate_b200.ops / vae_ops that has a stand-in above
+    is routed to it (or to `fakes[name]`, a test's own variant), the VAE's no-CPU guard `_require_cuda` is lifted (nothing
+    else of it), and decode_scaled writes its frames to host memory.  `mp` is a pytest.MonkeyPatch, which undoes all of it.
+    Its setattr raises AttributeError for a name the target module does not have, so renaming an entry point in the product
+    fails here rather than leaving the renamed one unreplaced."""
+    import easyanimate_b200.autoencoder_magvit as A
+    from easyanimate_b200 import ops, vae_ops
+    assert set(fakes) <= set(OPS + VAE_OPS), sorted(set(fakes) - set(OPS + VAE_OPS))
+    for module, names in ((ops, OPS), (vae_ops, VAE_OPS)):
+        for name in names:
+            mp.setattr(module, name, fakes.get(name, globals()[name]))
+    mp.setattr(A, "_require_cuda", lambda t, what: None)
+    mp.setattr(A.AutoencoderKLMagvit, "decode_scaled", _decode_scaled)

@@ -1,12 +1,12 @@
 """world_size-2 gloo test of the CFG-parallel host logic (rank -> branch assignment, all_gather layout, identical
 latents on both ranks, equality with the single-process batch-of-2 evaluation).  The transformer and the
 CFG+Euler kernel are replaced by CPU stand-ins: this exercises the N>1 plumbing, not the kernels."""
-import os
-
 import pytest
 import torch
 import torch.distributed as dist
-import torch.multiprocessing as mp
+
+from tests import cpu_ops
+from tests.gloo import run_ranks
 
 bf16 = torch.bfloat16
 
@@ -21,57 +21,26 @@ class FakeTransformer(torch.nn.Module):
         return (out.to(hidden_states.dtype),)
 
 
-def euler_cpu(noise_pred, latents, guidance_scale, sigma, sigma_next, use_cfg=True):
-    """torch restatement of ea_cfg_euler_step (pipeline_easyanimate.py:1102-1111) for the CPU test."""
-    if use_cfg:
-        u, c = noise_pred.chunk(2)
-        noise_pred = u + guidance_scale * (c - u)
-    dt = torch.tensor(sigma_next, dtype=torch.float32) - torch.tensor(sigma, dtype=torch.float32)
-    return (latents.float() + dt * noise_pred).to(noise_pred.dtype)
-
-
-def _inputs():
+def _sampler_run(cfg_group=None):
+    from easyanimate_b200.pipeline import EasyAnimateSampler
     g = torch.Generator().manual_seed(0)
-    return torch.randn(1, 4, 2, 4, 4, generator=g).to(bf16), torch.randn(2, 3, 8, generator=g).to(bf16)
+    lat, emb = torch.randn(1, 4, 2, 4, 4, generator=g).to(bf16), torch.randn(2, 3, 8, generator=g).to(bf16)
+    with pytest.MonkeyPatch.context() as mp:
+        cpu_ops.use_stand_ins(mp)
+        s = EasyAnimateSampler(FakeTransformer(), guidance_scale=6.0, cfg_group=cfg_group)
+        s.set_timesteps(4, device="cpu")
+        for i in range(4):
+            lat = s.step(lat, i, emb, None)
+    return lat.float()
 
 
-def _single():
-    from easyanimate_b200.pipeline import EasyAnimateSampler
-    lat, emb = _inputs()
-    s = EasyAnimateSampler(FakeTransformer(), guidance_scale=6.0, euler_fn=euler_cpu)
-    s.set_timesteps(4, device="cpu")
-    for i in range(4):
-        lat = s.step(lat, i, emb, None)
-    return lat
-
-
-def _worker(rank, port, q):
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE="2")
-    dist.init_process_group("gloo", rank=rank, world_size=2)
-    from easyanimate_b200.pipeline import EasyAnimateSampler
-    grp = dist.new_group([0, 1])
-    lat, emb = _inputs()
-    s = EasyAnimateSampler(FakeTransformer(), guidance_scale=6.0, cfg_group=grp, euler_fn=euler_cpu)
-    s.set_timesteps(4, device="cpu")
-    for i in range(4):
-        lat = s.step(lat, i, emb, None)
-    q.put((rank, lat.float()))
-    dist.barrier()
-    dist.destroy_process_group()
+def _cfg_pair(rank):
+    return _sampler_run(dist.new_group([0, 1]))
 
 
 def test_cfg_parallel_pair_matches_single_process():
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = 29500 + (os.getpid() % 400)
-    procs = [ctx.Process(target=_worker, args=(r, port, q)) for r in range(2)]
-    for p in procs:
-        p.start()
-    got = dict(q.get(timeout=120) for _ in range(2))
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
-    ref = _single().float()
+    got = run_ranks(_cfg_pair, 2, timeout=120)
+    ref = _sampler_run()
     assert torch.equal(got[0], got[1]), "both ranks of a CFG pair must hold identical latents"
     assert torch.equal(got[0], ref), "CFG-parallel must reproduce the batch-of-2 evaluation bit for bit"
 
@@ -104,18 +73,9 @@ _TC_CFG = dict(num_attention_heads=2, attention_head_dim=64, in_channels=33, out
 _TC_COEFFS = [1.07862322, -4.19362456, 3.06725828, 0.33161686, 0.02374758]
 
 
-def _install_cpu_ops():
-    from easyanimate_b200 import ops
-    from tests import cpu_ops
-    for name in ("gemm", "skinny_linear", "layernorm_modulate", "rmsnorm", "timestep_embedding", "patchify", "unpatchify",
-                 "qkv_gemm_ln_rope", "attention", "ew_add", "rel_l1_distance", "l1_sums"):
-        setattr(ops, name, getattr(cpu_ops, name))
-
-
 def _teacache_sampler_run(cfg_group=None, steps=8, thresh=0.15):
     """8 sampler steps with TeaCache on; returns (latents, skipped-forward count)."""
     from oracle import dit
-    from tests import cpu_ops
     from easyanimate_b200.pipeline import EasyAnimateSampler, rope_table
     from easyanimate_b200.transformer3d import EasyAnimateTransformer3DModel
     ob = dit.init_weights_(dit.OracleTransformer3D(**_TC_CFG), 11).to(bf16)
@@ -130,45 +90,25 @@ def _teacache_sampler_run(cfg_group=None, steps=8, thresh=0.15):
     # the joint-batch decision (with identical conditioning the per-branch means equal the joint mean and nothing is tested).
     inp = torch.cat([torch.zeros(1, 17, 3, 8, 12), torch.randn(1, 17, 3, 8, 12, generator=g) * 4.0]).to(bf16)
     rope = rope_table(64, 96, 3)
-    s = EasyAnimateSampler(m, guidance_scale=6.0, cfg_group=cfg_group, euler_fn=cpu_ops.cfg_euler_step)
-    s.set_timesteps(steps, device="cpu")
-    with torch.no_grad():
+    with pytest.MonkeyPatch.context() as mp, torch.no_grad():
+        cpu_ops.use_stand_ins(mp)
+        s = EasyAnimateSampler(m, guidance_scale=6.0, cfg_group=cfg_group)
+        s.set_timesteps(steps, device="cpu")
         for i in range(steps):
             lat = s.step(lat, i, emb, rope, inpaint_latents=inp)
     return lat.float(), m.teacache.skipped
 
 
-def _teacache_worker(rank, port, q):
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE="2")
-    dist.init_process_group("gloo", rank=rank, world_size=2)
-    _install_cpu_ops()
-    out, skipped = _teacache_sampler_run(dist.new_group([0, 1]))
-    q.put((rank, out, skipped))
-    dist.barrier()
-    dist.destroy_process_group()
+def _teacache_cfg_pair(rank):
+    return _teacache_sampler_run(dist.new_group([0, 1]))
 
 
 def test_teacache_with_cfg_parallel_takes_the_joint_batch_decision():
     """With cfg_group each rank sees one branch (B=1); the reference decides skip/compute once per step
     from the rel-L1 means over the batch of 2 (transformer3d.py:1563-1586).  The (num, den) sums are all-reduced over the
     CFG pair, so both ranks skip exactly where the single-process batch-of-2 run skips and the latents agree bit for bit."""
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = 29900 + (os.getpid() % 90)
-    procs = [ctx.Process(target=_teacache_worker, args=(r, port, q)) for r in range(2)]
-    for p in procs:
-        p.start()
-    res = dict((r, (o, s)) for r, o, s in (q.get(timeout=180) for _ in range(2)))
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
-    _install_cpu_ops()
-    try:
-        single, skipped = _teacache_sampler_run(None)
-    finally:
-        import importlib
-        from easyanimate_b200 import ops
-        importlib.reload(ops)
+    res = run_ranks(_teacache_cfg_pair, 2, timeout=180)
+    single, skipped = _teacache_sampler_run(None)
     assert skipped >= 1, "the test must exercise the cached path"
     assert res[0][1] == res[1][1] == skipped, (res[0][1], res[1][1], skipped)
     assert torch.equal(res[0][0], res[1][0]) and torch.equal(res[0][0], single)
@@ -198,42 +138,25 @@ class _PipeVae(torch.nn.Module):
 
 
 def _pipeline_call(cfg_group=None):
-    from easyanimate_b200 import ops
     from easyanimate_b200.pipelines import EasyAnimatePipeline
     g = torch.Generator().manual_seed(3)
     pe, ne = torch.randn(1, 3, 8, generator=g).to(bf16), torch.randn(1, 3, 8, generator=g).to(bf16)
     ones = torch.ones(1, 3, dtype=torch.long)
     pipe = EasyAnimatePipeline(vae=_PipeVae(), transformer=_PipeTransformer(), cfg_group=cfg_group)
-    real, ops.cfg_euler_step = ops.cfg_euler_step, euler_cpu  # the sampler binds the CFG + Euler kernel at construction
-    try:
+    with pytest.MonkeyPatch.context() as mp:
+        cpu_ops.use_stand_ins(mp)
         return pipe(video_length=5, height=32, width=32, num_inference_steps=3, guidance_scale=6.0,
                     generator=torch.Generator().manual_seed(4), prompt_embeds=pe, negative_prompt_embeds=ne,
                     prompt_attention_mask=ones, negative_prompt_attention_mask=ones, prompt_embeds_2=pe,
                     prompt_attention_mask_2=ones).frames
-    finally:
-        ops.cfg_euler_step = real
 
 
-def _pipe_worker(rank, port, q):
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE="2")
-    dist.init_process_group("gloo", rank=rank, world_size=2)
-    frames = _pipeline_call(dist.new_group([0, 1]))
-    q.put((rank, frames))
-    dist.barrier()
-    dist.destroy_process_group()
+def _pipeline_cfg_pair(rank):
+    return _pipeline_call(dist.new_group([0, 1]))
 
 
 def test_native_pipeline_call_on_a_cfg_pair_matches_single_process():
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = 30100 + (os.getpid() % 400)
-    procs = [ctx.Process(target=_pipe_worker, args=(r, port, q)) for r in range(2)]
-    for p in procs:
-        p.start()
-    got = dict(q.get(timeout=120) for _ in range(2))
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
+    got = run_ranks(_pipeline_cfg_pair, 2, timeout=120)
     ref = _pipeline_call()
     assert ref.shape == (1, 3, 2, 4, 4)
     assert torch.equal(got[0], got[1]) and torch.equal(got[0], ref)

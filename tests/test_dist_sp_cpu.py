@@ -1,11 +1,12 @@
 """world_size-2 gloo check of the Ulysses sequence-parallel exchanges (easyanimate_b200/sequence_parallel.py): head scatter /
 token gather before attention, the reverse after it, the replicated text rows, and the token shard / gather of the
 per-token streams - against single-process attention over all tokens.  Attention itself is a CPU stand-in."""
-import os
-
+import pytest
 import torch
 import torch.distributed as dist
-import torch.multiprocessing as mp
+
+from tests import cpu_ops
+from tests.gloo import run_ranks
 
 B, H, S_T, S_V = 2, 4, 5, 12
 
@@ -21,39 +22,28 @@ def _global_qkv():
     return [torch.randn(B, H, S_T + S_V, 64, generator=g) for _ in range(3)]
 
 
-def _worker(rank, port, q_out):
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE="2")
-    dist.init_process_group("gloo", rank=rank, world_size=2)
+def _exchanges(rank):
     from easyanimate_b200.sequence_parallel import UlyssesAttention
-    sp = UlyssesAttention(dist.new_group([0, 1]), attention_fn=_attention_cpu)
+    sp = UlyssesAttention(dist.new_group([0, 1]))
     s0, s1 = sp.local_range(S_V)
     q, k, v = _global_qkv()
     local = [torch.cat([t[:, :, :S_T], t[:, :, S_T + s0:S_T + s1]], dim=2).contiguous() for t in (q, k, v)]
-    o_t, o_v = sp.attention(local[0], local[1], local[2], S_T)
+    with pytest.MonkeyPatch.context() as mp:
+        cpu_ops.use_stand_ins(mp, attention=_attention_cpu)
+        o_t, o_v = sp.attention(local[0], local[1], local[2], S_T)
     # token shard / gather round trip of a per-token stream
     x = torch.arange(B * S_V * 3, dtype=torch.float32).view(B * S_V, 3)
     x_loc = sp.shard_tokens(x, B, S_V)
     back = sp.gather_tokens(x_loc, B, s1 - s0)
-    q_out.put((rank, o_t, o_v, bool(torch.equal(back, x)), tuple(x_loc.shape)))
-    dist.barrier()
-    dist.destroy_process_group()
+    return o_t, o_v, bool(torch.equal(back, x)), tuple(x_loc.shape)
 
 
 def test_ulysses_exchanges_match_single_process_attention():
-    ctx = mp.get_context("spawn")
-    q_out = ctx.Queue()
-    port = 29700 + (os.getpid() % 90)
-    procs = [ctx.Process(target=_worker, args=(r, port, q_out)) for r in range(2)]
-    for p in procs:
-        p.start()
-    res = sorted([q_out.get(timeout=120) for _ in range(2)], key=lambda r: r[0])
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
+    res = run_ranks(_exchanges, 2, timeout=120)
     q, k, v = _global_qkv()
     full_t, full_v = _attention_cpu(q, k, v, S_T)
     n = S_V // 2
-    for rank, o_t, o_v, roundtrip, shape in res:
+    for rank, (o_t, o_v, roundtrip, shape) in enumerate(res):
         assert roundtrip and shape == (B * n, 3)
         torch.testing.assert_close(o_t, full_t, rtol=1e-5, atol=1e-6)
         torch.testing.assert_close(o_v, full_v[:, rank * n:(rank + 1) * n], rtol=1e-5, atol=1e-6)
@@ -62,14 +52,6 @@ def test_ulysses_exchanges_match_single_process_attention():
 # ---- the whole transformer forward under sequence parallelism (host logic; CUDA entry points replaced by tests/cpu_ops.py) ----
 CFG = dict(num_attention_heads=2, attention_head_dim=64, in_channels=16, out_channels=16, patch_size=2, num_layers=2,
            time_embed_dim=64, add_norm_text_encoder=True, text_embed_dim=128, text_embed_dim_t5=None)
-
-
-def _install_cpu_ops():
-    from easyanimate_b200 import ops
-    from tests import cpu_ops
-    for name in ("gemm", "skinny_linear", "layernorm_modulate", "rmsnorm", "timestep_embedding", "patchify", "unpatchify",
-                 "qkv_gemm_ln_rope", "attention", "ew_add", "rel_l1_distance", "l1_sums"):
-        setattr(ops, name, getattr(cpu_ops, name))
 
 
 def _forward(sp_group=None, teacache=False):
@@ -85,7 +67,8 @@ def _forward(sp_group=None, teacache=False):
     enc = (torch.randn(2, 9, 128, generator=g) * 3).to(bf16)
     t = torch.tensor([937.0, 421.0]).to(bf16)
     rope = dit.rope_for_video(64, 96, 3)
-    with torch.no_grad():
+    with pytest.MonkeyPatch.context() as mp, torch.no_grad():
+        cpu_ops.use_stand_ins(mp)
         if not teacache:
             return m(lat, t, encoder_hidden_states=enc, image_rotary_emb=rope, return_dict=False)[0]
         m.enable_teacache(6, 0.08, coefficients=[1.07862322, -4.19362456, 3.06725828, 0.33161686, 0.02374758])
@@ -97,49 +80,26 @@ def _forward(sp_group=None, teacache=False):
         return torch.stack(outs)
 
 
-def _model_worker(rank, port, q_out):
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE="2")
-    dist.init_process_group("gloo", rank=rank, world_size=2)
-    _install_cpu_ops()
+def _sp_forwards(rank):
     grp = dist.new_group([0, 1])
-    out = _forward(grp)
-    out_tc = _forward(grp, teacache=True)
-    q_out.put((rank, out.float(), out_tc.float()))
-    dist.barrier()
-    dist.destroy_process_group()
+    return _forward(grp).float(), _forward(grp, teacache=True).float()
 
 
 def test_sequence_parallel_forward_equals_single_process_forward():
-    ctx = mp.get_context("spawn")
-    q_out = ctx.Queue()
-    port = 29800 + (os.getpid() % 90)
-    procs = [ctx.Process(target=_model_worker, args=(r, port, q_out)) for r in range(2)]
-    for p in procs:
-        p.start()
-    res = sorted([q_out.get(timeout=180) for _ in range(2)], key=lambda r: r[0])
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
-    _install_cpu_ops()
-    try:
-        single = _forward(None).float()
-        single_tc = _forward(None, teacache=True).float()
-    finally:
-        import importlib
-        from easyanimate_b200 import ops
-        importlib.reload(ops)  # put the real entry points back for the rest of the session
+    res = run_ranks(_sp_forwards, 2, timeout=180)
+    single = _forward(None).float()
+    single_tc = _forward(None, teacache=True).float()
     # every per-token op sees the same rows and attention sees the same keys: identical, not just close
-    assert torch.equal(res[0][1], res[1][1])
-    assert torch.equal(res[0][1], single)
+    assert torch.equal(res[0][0], res[1][0])
+    assert torch.equal(res[0][0], single)
     # TeaCache under sequence parallelism: the rel-L1 pieces are summed over the group, so every rank takes the same
     # skip decisions as the single-process run (6 calls, at least one served from the cached residual)
-    assert torch.equal(res[0][2], res[1][2]) and torch.equal(res[0][2], single_tc)
+    assert torch.equal(res[0][1], res[1][1]) and torch.equal(res[0][1], single_tc)
 
 
 # ---- one video on 4 ranks: 2 CFG branches x 2 sequence-parallel ranks (the 8-GPU single-video topology at small scale) ----
 def _sampler_run(sp_group=None, cfg_group=None):
     from oracle import dit
-    from tests import cpu_ops
     from easyanimate_b200.pipeline import EasyAnimateSampler
     from easyanimate_b200.transformer3d import EasyAnimateTransformer3DModel
     bf16 = torch.bfloat16
@@ -152,43 +112,23 @@ def _sampler_run(sp_group=None, cfg_group=None):
     emb = (torch.randn(2, 9, 128, generator=g) * 3).to(bf16)  # cat(negative, positive)
     from easyanimate_b200.pipeline import rope_table
     rope = rope_table(64, 96, 3)
-    s = EasyAnimateSampler(m, guidance_scale=6.0, cfg_group=cfg_group, euler_fn=cpu_ops.cfg_euler_step)
-    s.set_timesteps(3, device="cpu")
-    with torch.no_grad():
+    with pytest.MonkeyPatch.context() as mp, torch.no_grad():
+        cpu_ops.use_stand_ins(mp)
+        s = EasyAnimateSampler(m, guidance_scale=6.0, cfg_group=cfg_group)
+        s.set_timesteps(3, device="cpu")
         for i in range(3):
             lat = s.step(lat, i, emb, rope)
     return lat.float()
 
 
-def _topology_worker(rank, port, q_out):
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE="4")
-    dist.init_process_group("gloo", rank=rank, world_size=4)
-    _install_cpu_ops()
+def _cfg_pairs_times_sp(rank):
     sp_groups = [dist.new_group([0, 1]), dist.new_group([2, 3])]      # every rank creates every group
     cfg_pairs = [dist.new_group([0, 2]), dist.new_group([1, 3])]      # rank r (uncond branch) <-> rank r + 2 (text branch)
-    out = _sampler_run(sp_group=sp_groups[rank // 2], cfg_group=cfg_pairs[rank % 2])
-    q_out.put((rank, out))
-    dist.barrier()
-    dist.destroy_process_group()
+    return _sampler_run(sp_group=sp_groups[rank // 2], cfg_group=cfg_pairs[rank % 2])
 
 
 def test_cfg_pairs_times_sequence_parallel_equals_single_process_sampler():
-    ctx = mp.get_context("spawn")
-    q_out = ctx.Queue()
-    port = 29500 + (os.getpid() % 90)
-    procs = [ctx.Process(target=_topology_worker, args=(r, port, q_out)) for r in range(4)]
-    for p in procs:
-        p.start()
-    res = sorted([q_out.get(timeout=300) for _ in range(4)], key=lambda r: r[0])
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
-    _install_cpu_ops()
-    try:
-        single = _sampler_run()
-    finally:
-        import importlib
-        from easyanimate_b200 import ops
-        importlib.reload(ops)
-    for rank, out in res:
+    res = run_ranks(_cfg_pairs_times_sp, 4, timeout=300)
+    single = _sampler_run()
+    for rank, out in enumerate(res):
         assert torch.equal(out, single), rank

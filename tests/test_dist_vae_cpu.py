@@ -1,10 +1,11 @@
 """world_size-2 gloo check of the VAE tile-parallel plumbing (partition of the reference's tiled_decode tiles over
 ranks, padding, all-gather layout, reassembly order) with CPU stand-ins for the decoder pass and the copy kernel."""
-import os
-
+import pytest
 import torch
 import torch.distributed as dist
-import torch.multiprocessing as mp
+
+from tests import cpu_ops
+from tests.gloo import run_ranks
 
 bf16 = torch.bfloat16
 
@@ -15,58 +16,31 @@ def _fake_decode(self, zt):  # [C,T,h,w] -> [1,3,T',8h,8w]: deterministic functi
     return (base[None, None].expand(1, 3, 4 * (T - 1) + 1, 8 * h, 8 * w) + 1.0).to(bf16).contiguous()
 
 
-def _copy_cpu(src, dst, rows, cols, r0, c0):
-    dst[..., r0:r0 + rows, c0:c0 + cols] = src[..., :rows, :cols]
-
-
-def _tile_worker(rank, port, q):
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE="2")
-    dist.init_process_group("gloo", rank=rank, world_size=2)
-    from easyanimate_b200 import vae_ops
+def _tile_layout(rank):
     from easyanimate_b200.autoencoder_magvit import AutoencoderKLMagvit
-
-    AutoencoderKLMagvit._decode_one = _fake_decode
-    vae_ops.copy2d = _copy_cpu
     m = AutoencoderKLMagvit(latent_channels=16, cache_mag_vae=True, spatial_group_norm=True, mid_block_attention_type="spatial",
                             block_out_channels=[64, 64, 128, 128], use_tiling=True, tile_sample_min_size=64)
     z = torch.randn(16, 2, 14, 20, generator=torch.Generator().manual_seed(3)).to(bf16)
     tl, ov = m.tile_latent_min_size, int(m.tile_latent_min_size * 0.75)
     coords = [[(i, j) for j in range(0, 20, ov)] for i in range(0, 14, ov)]
-    rows, corner = m._decode_tiles_parallel(z, coords, tl, dist.new_group([0, 1]))
+    with pytest.MonkeyPatch.context() as mp:
+        cpu_ops.use_stand_ins(mp)
+        mp.setattr(AutoencoderKLMagvit, "_decode_one", _fake_decode)
+        rows, corner = m._decode_tiles_parallel(z, coords, tl, dist.new_group([0, 1]))
     ok = True
     for row_c, row_t in zip(coords, rows):
         for (i, j), t in zip(row_c, row_t):
             ok &= torch.equal(t, _fake_decode(m, z[:, :, i:i + tl, j:j + tl]))
     ok &= torch.equal(corner, _fake_decode(m, z[:, :, -tl:, -tl:]))
-    q.put((rank, bool(ok), len(rows), len(rows[0])))
-    dist.barrier()
-    dist.destroy_process_group()
+    return bool(ok), len(rows), len(rows[0])
 
 
 def test_vae_tile_parallel_gather_reassembles_every_tile():
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = 29900 + (os.getpid() % 90)
-    procs = [ctx.Process(target=_tile_worker, args=(r, port, q)) for r in range(2)]
-    for p in procs:
-        p.start()
-    res = [q.get(timeout=120) for _ in range(2)]
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
-    assert all(r[1] for r in res) and res[0][2:] == (3, 4), res
+    res = run_ranks(_tile_layout, 2, timeout=120)
+    assert all(r[0] for r in res) and res[0][1:] == (3, 4), res
 
 
 # ---- the real module (all decoder layers, blending, corner pass) with torch stand-ins for the kernels (tests/cpu_ops.py) ----
-def _install_cpu_vae_ops():
-    from easyanimate_b200 import ops, vae_ops
-    from tests import cpu_ops
-    for name in ("conv3d_causal", "prepare_latents", "groupnorm", "upsample2x", "spatial_attention", "tile_blend", "copy2d",
-                 "corner_blend"):
-        setattr(vae_ops, name, getattr(cpu_ops, name))
-    ops.gemm = cpu_ops.gemm
-
-
 def _real_decode(group):
     from oracle import vae
     from easyanimate_b200.autoencoder_magvit import AutoencoderKLMagvit
@@ -76,45 +50,32 @@ def _real_decode(group):
                             block_out_channels=boc, use_tiling=True, tile_sample_min_size=64).to(bf16)
     m.load_state_dict({k: v.to(bf16) for k, v in ob.state_dict().items()}, strict=False)
     m.set_tile_parallel_group(group)
-    z = torch.randn(16, 2, 14, 13, generator=torch.Generator().manual_seed(6)).to(bf16)
-    with torch.no_grad():
-        return m._tiled_decode_one(z)
+    z = torch.randn(1, 16, 2, 14, 13, generator=torch.Generator().manual_seed(6)).to(bf16)
+    with pytest.MonkeyPatch.context() as mp:
+        cpu_ops.use_stand_ins(mp)
+        return m.decode(z).sample.float()
 
 
-def _real_worker(rank, port, q):
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE="2")
-    dist.init_process_group("gloo", rank=rank, world_size=2)
-    _install_cpu_vae_ops()
-    out = _real_decode(dist.new_group([0, 1]))
-    q.put((rank, out.float()))
-    dist.barrier()
-    dist.destroy_process_group()
+def _tile_parallel_decode(rank):
+    return _real_decode(dist.new_group([0, 1]))
 
 
 def test_vae_tile_parallel_decode_equals_single_process_tiled_decode():
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = 29600 + (os.getpid() % 90)
-    procs = [ctx.Process(target=_real_worker, args=(r, port, q)) for r in range(2)]
-    for p in procs:
-        p.start()
-    res = sorted([q.get(timeout=300) for _ in range(2)], key=lambda r: r[0])
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
-    import importlib
-    from easyanimate_b200 import ops, vae_ops
-    _install_cpu_vae_ops()
-    try:
-        single = _real_decode(None).float()
-    finally:
-        importlib.reload(ops)
-        importlib.reload(vae_ops)
+    res = run_ranks(_tile_parallel_decode, 2, timeout=300)
+    single = _real_decode(None)
     assert single.shape == (1, 3, 5, 112, 104)
-    assert torch.equal(res[0][1], res[1][1]) and torch.equal(res[0][1], single)
+    assert torch.equal(res[0], res[1]) and torch.equal(res[0], single)
 
 
 # ---- strip-parallel UNTILED decode (easyanimate_b200/vae_strips.py): halo rows, gathered GroupNorm sums, gathered frames ----
+def groupnorm_one_part(x, gamma, beta, groups, eps, silu):
+    # the single-process decode through the SAME stand-in arithmetic as the strips (on the GPU both forms end in the same
+    # apply kernel; F.group_norm rounds differently from the explicit (x - mean) * rstd form)
+    T, H, W, C = x.shape
+    return cpu_ops.groupnorm_from_sums(x, cpu_ops.groupnorm_sums(x, groups)[None], float(H * W * (C // groups)), gamma, beta,
+                                       groups, eps, silu)
+
+
 def _strip_decode(group, h=11, w=6):
     from oracle import vae
     from easyanimate_b200.autoencoder_magvit import AutoencoderKLMagvit
@@ -123,52 +84,15 @@ def _strip_decode(group, h=11, w=6):
     m = AutoencoderKLMagvit(latent_channels=16, cache_mag_vae=True, spatial_group_norm=True, mid_block_attention_type="spatial",
                             block_out_channels=boc).to(bf16)
     m.load_state_dict({k: v.to(bf16) for k, v in ob.state_dict().items()}, strict=False)
-    z = torch.randn(16, 2, h, w, generator=torch.Generator().manual_seed(8)).to(bf16)
-    with torch.no_grad():  # (decode() itself refuses CPU tensors: the two branches of _decode are called directly)
-        if group is None:
-            return m._decode_one(z)
-        from easyanimate_b200.vae_strips import decode_strips
-        return decode_strips(m, z, group)
+    m.set_strip_parallel_group(group)
+    z = torch.randn(1, 16, 2, h, w, generator=torch.Generator().manual_seed(8)).to(bf16)
+    with pytest.MonkeyPatch.context() as mp:
+        cpu_ops.use_stand_ins(mp, groupnorm=groupnorm_one_part)
+        return m.decode(z).sample.float()
 
 
-def _install_cpu_strip_ops():
-    from easyanimate_b200 import vae_ops
-    from tests import cpu_ops
-    _install_cpu_vae_ops()
-    for name in ("groupnorm_sums", "groupnorm_from_sums"):
-        setattr(vae_ops, name, getattr(cpu_ops, name))
-
-    def groupnorm_one_part(x, gamma, beta, groups, eps, silu):
-        # the single-process decode through the SAME stand-in arithmetic as the strips (on the GPU both forms end in the same
-        # apply kernel; F.group_norm rounds differently from the explicit (x - mean) * rstd form)
-        T, H, W, C = x.shape
-        return cpu_ops.groupnorm_from_sums(x, cpu_ops.groupnorm_sums(x, groups)[None], float(H * W * (C // groups)), gamma, beta,
-                                           groups, eps, silu)
-    vae_ops.groupnorm = groupnorm_one_part
-
-
-def _strip_worker(rank, world, port, q):
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world))
-    dist.init_process_group("gloo", rank=rank, world_size=world)
-    _install_cpu_strip_ops()
-    out = _strip_decode(dist.new_group(list(range(world))))
-    q.put((rank, out.float()))
-    dist.barrier()
-    dist.destroy_process_group()
-
-
-def _run_strips(world):
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = 29700 + (os.getpid() % 90) + world
-    procs = [ctx.Process(target=_strip_worker, args=(r, world, port, q)) for r in range(world)]
-    for p in procs:
-        p.start()
-    res = sorted([q.get(timeout=300) for _ in range(world)], key=lambda r: r[0])
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
-    return [r[1] for r in res]
+def _strip_parallel_decode(rank, world):
+    return _strip_decode(dist.new_group(list(range(world))))
 
 
 def test_vae_strip_parallel_decode_equals_single_process_untiled_decode():
@@ -178,17 +102,10 @@ def test_vae_strip_parallel_decode_equals_single_process_untiled_decode():
     first up-sampled convolution on, PyTorch's CPU conv3d blocks a strip-shaped input differently from the full frame (fp32
     summation order), which flips a few bf16 roundings that a random-init network then spreads - hence a tolerance here.  On
     the GPU the convolution's k order does not depend on the strip (tools/test_multigpu.py checks that decode)."""
-    import importlib
-    from easyanimate_b200 import ops, vae_ops
-    _install_cpu_strip_ops()
-    try:
-        single = _strip_decode(None).float()
-    finally:
-        importlib.reload(ops)
-        importlib.reload(vae_ops)
+    single = _strip_decode(None)
     assert single.shape == (1, 3, 5, 88, 48)
     for world in (2, 3):
-        outs = _run_strips(world)
+        outs = run_ranks(_strip_parallel_decode, world, world, timeout=300)
         for o in outs[1:]:
             assert torch.equal(o, outs[0])
         diff = (outs[0] - single).abs()

@@ -2,8 +2,6 @@
 restated in tests/long_video_oracle.py over the reference's own EasyAnimateInpaintPipeline, PIL for the chained frames), both
 over the same tiny product modules with the kernels replaced by the torch stand-ins of tests/cpu_ops.py.  Where the reference is
 not installed the frames are compared with a stored sample of the reference's (tests/golden/long_video_ref.safetensors)."""
-import os
-
 import numpy as np
 import pytest
 import torch
@@ -11,30 +9,14 @@ from PIL import Image
 
 from oracle import ref_pipeline
 from tests import cpu_ops, long_video_oracle, refgold
-from tests.test_native_pipelines_cpu import _embeds, _mask_kw, _modules, on_cpu  # noqa: F401  (on_cpu is a fixture)
+from tests.gloo import run_ranks
+from tests.test_native_pipelines_cpu import _embeds, _mask_kw, _modules
 
 LIVE = ref_pipeline.available()
 GOLD = refgold.Store("long_video_ref")
 H, W, STEPS = 64, 96, 2
 INP = dict(in_channels=33, seeds=(73, 74), resize_inpaint_mask_directly=True, enable_clip_in_inpaint=False,
            add_noise_in_inpaint_model=True)
-
-
-def frames_out_blend(video, out, overlap):
-    """ea_frames_out_blend as the reference's tensor ops (pipeline_easyanimate.py:738-741, then ui.py:524-531)."""
-    f = (video.clamp(-1, 1) / 2 + 0.5).clamp(0, 1).float()
-    if overlap:
-        r = torch.tensor([float(i) / float(overlap) for i in range(overlap)], dtype=torch.float32).view(1, 1, -1, 1, 1)
-        out[:, :, :overlap] = out[:, :, :overlap] * (1 - r) + f[:, :, :overlap] * r
-    out[:, :, overlap:] = f[:, :, overlap:]
-    return out
-
-
-@pytest.fixture
-def lv_cpu(on_cpu, monkeypatch):  # noqa: F811
-    from easyanimate_b200 import vae_ops
-    monkeypatch.setattr(vae_ops, "frames_out_blend", frames_out_blend)
-    return on_cpu
 
 
 @pytest.fixture(scope="module", autouse=True)
@@ -57,10 +39,11 @@ CASES = {  # name: (video_length, partial_video_length, overlap_video_length, st
 
 
 @pytest.mark.parametrize("case", sorted(CASES))
-def test_long_video_equals_the_reference_loop(lv_cpu, case):
+def test_long_video_equals_the_reference_loop(monkeypatch, case):
     from easyanimate_b200 import EasyAnimateInpaintPipeline, generate_long_video
+    cpu_ops.use_stand_ins(monkeypatch)
     length, partial, ov, n_start, n_end = CASES[case]
-    t, v = _modules(lv_cpu, **INP)
+    t, v = _modules(**INP)
     pe, ne = _embeds(torch.Generator().manual_seed(50))
     start = None if n_start is None else _images(51, n_start)
     end = None if n_end is None else _images(52, n_end)
@@ -96,10 +79,11 @@ def test_window_schedule_equals_the_reference_loop():
     assert long_video_windows(97, 49, 4) == [(0, 49), (45, 49), (90, 5)]
 
 
-def test_long_video_refuses_what_the_reference_refuses(lv_cpu):
+def test_long_video_refuses_what_the_reference_refuses(monkeypatch):
     from easyanimate_b200 import EasyAnimateInpaintPipeline, EasyAnimatePipeline, generate_long_video
-    t, v = _modules(lv_cpu, **INP)
-    t16, _ = _modules(lv_cpu)
+    cpu_ops.use_stand_ins(monkeypatch)
+    t, v = _modules(**INP)
+    t16, _ = _modules()
     pe, ne = _embeds(torch.Generator().manual_seed(54))
     ok = dict(video_length=13, partial_video_length=9, height=H, width=W, num_inference_steps=STEPS, guidance_scale=6.0,
               **_mask_kw(pe, ne))
@@ -119,10 +103,11 @@ def test_long_video_refuses_what_the_reference_refuses(lv_cpu):
             generate_long_video(pipe, **{**ok, **extra})
 
 
-def test_tensor_images_condition_like_pil_images(lv_cpu):
+def test_tensor_images_condition_like_pil_images(monkeypatch):
     """uint8 tensors [n,3,H,W] give the frames the same pictures give as PIL images."""
     from easyanimate_b200 import EasyAnimateInpaintPipeline, generate_long_video
-    t, v = _modules(lv_cpu, **INP)
+    cpu_ops.use_stand_ins(monkeypatch)
+    t, v = _modules(**INP)
     pe, ne = _embeds(torch.Generator().manual_seed(56))
     start, end = _images(57, 2), _images(58, 1)
     as_tensor = [torch.stack([torch.from_numpy(np.array(im)).permute(2, 0, 1) for im in ims]) for ims in (start, end)]
@@ -135,53 +120,27 @@ def test_tensor_images_condition_like_pil_images(lv_cpu):
     assert torch.equal(a, b)
 
 
-def _dist_worker(rank, port, q):
-    import torch.distributed as dist
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE="2")
-    dist.init_process_group("gloo", rank=rank, world_size=2)
-    mp = pytest.MonkeyPatch()
-    try:
-        q.put((rank, _run_cfg_pair(mp, dist.new_group([0, 1]))))
-        dist.barrier()
-    finally:
-        mp.undo()
-        dist.destroy_process_group()
-
-
-def _run_cfg_pair(mp, group):
-    import easyanimate_b200.autoencoder_magvit as A
-    from easyanimate_b200 import EasyAnimateInpaintPipeline, generate_long_video, ops, vae_ops
-    cpu_ops.install(mp)
-    cpu_ops.install_vae(mp)
-    mp.setattr(ops, "cfg_euler_step", cpu_ops.cfg_euler_step)
-    mp.setattr(A, "_require_cuda", lambda t, what: None)
-    mp.setattr(vae_ops, "frames_out_blend", frames_out_blend)
-    t, v = _modules(A, **INP)
+def _run_cfg_pair(group=None):
+    from easyanimate_b200 import EasyAnimateInpaintPipeline, generate_long_video
+    t, v = _modules(**INP)
     pe, ne = _embeds(torch.Generator().manual_seed(60))
     pipe = EasyAnimateInpaintPipeline(vae=v, transformer=t, cfg_group=group)
-    return generate_long_video(pipe, video_length=13, partial_video_length=9, overlap_video_length=4, start_image=_images(61, 1),
-                               height=H, width=W, num_inference_steps=STEPS, guidance_scale=6.0,
-                               generator=torch.Generator().manual_seed(62), **_mask_kw(pe, ne)).frames
+    with pytest.MonkeyPatch.context() as mp:
+        cpu_ops.use_stand_ins(mp)
+        return generate_long_video(pipe, video_length=13, partial_video_length=9, overlap_video_length=4,
+                                   start_image=_images(61, 1), height=H, width=W, num_inference_steps=STEPS, guidance_scale=6.0,
+                                   generator=torch.Generator().manual_seed(62), **_mask_kw(pe, ne)).frames
+
+
+def _cfg_pair(rank):
+    import torch.distributed as dist
+    return _run_cfg_pair(dist.new_group([0, 1]))
 
 
 def test_cfg_parallel_pair_gives_the_single_process_video():
     """A gloo CFG pair (each rank one guidance branch, pipeline.py): both ranks return the whole video, equal to one process."""
-    import torch.multiprocessing as tmp
-    ctx = tmp.get_context("spawn")
-    q = ctx.Queue()
-    port = 29100 + (os.getpid() % 400)
-    procs = [ctx.Process(target=_dist_worker, args=(r, port, q)) for r in range(2)]
-    for p in procs:
-        p.start()
-    got = dict(q.get(timeout=600) for _ in range(2))
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
-    mp = pytest.MonkeyPatch()
-    try:
-        single = _run_cfg_pair(mp, None)
-    finally:
-        mp.undo()
+    got = run_ranks(_cfg_pair, 2, timeout=600)
+    single = _run_cfg_pair()
     assert torch.equal(got[0], got[1]) and torch.equal(got[0], single)
 
 

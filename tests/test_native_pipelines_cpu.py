@@ -21,28 +21,13 @@ BOC = (64, 64, 128, 128)
 H, W, FRAMES, LF, STEPS = 64, 96, 5, 2, 3
 
 
-@pytest.fixture
-def on_cpu(monkeypatch):
-    import easyanimate_b200.autoencoder_magvit as A
-    from easyanimate_b200 import ops
-    cpu_ops.install(monkeypatch)
-    cpu_ops.install_vae(monkeypatch)
-    monkeypatch.setattr(ops, "cfg_euler_step", cpu_ops.cfg_euler_step)
-    monkeypatch.setattr(A, "_require_cuda", lambda t, what: None)
-
-    def decode_scaled(self, latents, out=None, dtype=torch.float32, to_host=False):  # no pinned memory / stream on this box
-        self._latent_in_scale = 1.0 / float(self.config.scaling_factor)
-        try:
-            video = self._decode(latents)
-        finally:
-            self._latent_in_scale = 1.0
-        return cpu_ops.frames_out(video.contiguous(), torch.empty(video.shape, dtype=dtype))
-
-    monkeypatch.setattr(A.AutoencoderKLMagvit, "decode_scaled", decode_scaled)
-    return A
+@pytest.fixture(autouse=True)
+def _stand_ins(monkeypatch):
+    cpu_ops.use_stand_ins(monkeypatch)
 
 
-def _modules(A, in_channels=16, seeds=(71, 72), **flags):
+def _modules(in_channels=16, seeds=(71, 72), **flags):
+    from easyanimate_b200.autoencoder_magvit import AutoencoderKLMagvit
     from easyanimate_b200.transformer3d import EasyAnimateTransformer3DModel
     cfg = dict(CFG, in_channels=in_channels, **flags)
     ocfg = {k: v for k, v in cfg.items() if k not in flags and k != "time_position_encoding_type"}
@@ -50,8 +35,8 @@ def _modules(A, in_channels=16, seeds=(71, 72), **flags):
     t = EasyAnimateTransformer3DModel(**cfg).to(bf16)
     t.load_state_dict(ob.state_dict(), strict=True)
     ov = vae.init_weights_(vae.OracleAutoencoderKLMagvit(block_out_channels=list(BOC), with_encoder=True), seeds[1]).to(bf16)
-    v = A.AutoencoderKLMagvit(latent_channels=16, cache_mag_vae=True, spatial_group_norm=True, mid_block_attention_type="spatial",
-                              block_out_channels=list(BOC), scaling_factor=0.7125, mini_batch_encoder=4, mini_batch_decoder=1).to(bf16)
+    v = AutoencoderKLMagvit(latent_channels=16, cache_mag_vae=True, spatial_group_norm=True, mid_block_attention_type="spatial",
+                            block_out_channels=list(BOC), scaling_factor=0.7125, mini_batch_encoder=4, mini_batch_decoder=1).to(bf16)
     v.load_state_dict(ov.state_dict(), strict=True)
     return t, v
 
@@ -87,9 +72,9 @@ def _live(fn):
     return fn if LIVE else None
 
 
-def test_t2v_pipeline_equals_the_reference_pipeline(on_cpu):
+def test_t2v_pipeline_equals_the_reference_pipeline():
     from easyanimate_b200 import EasyAnimatePipeline
-    t, v = _modules(on_cpu)
+    t, v = _modules()
     g = torch.Generator().manual_seed(1)
     lat = torch.randn(1, 16, LF, H // 8, W // 8, generator=g).to(bf16)
     pe, ne = _embeds(g)
@@ -112,9 +97,9 @@ def test_t2v_pipeline_equals_the_reference_pipeline(on_cpu):
                                                             guidance_scale=1.0, latents=lat, **_mask_kw(pe, ne)).frames)
 
 
-def test_t2v_pipeline_rejects_what_the_reference_rejects(on_cpu):
+def test_t2v_pipeline_rejects_what_the_reference_rejects():
     from easyanimate_b200 import EasyAnimatePipeline
-    t, v = _modules(on_cpu)
+    t, v = _modules()
     pipe = EasyAnimatePipeline(vae=v, transformer=t)
     g = torch.Generator().manual_seed(2)
     pe, ne = _embeds(g)
@@ -140,9 +125,9 @@ def test_t2v_pipeline_rejects_what_the_reference_rejects(on_cpu):
         pipe(**ok, **_mask_kw(pe, ne), guidance_rescale=0.7)
 
 
-def test_callback_on_step_end_sees_and_replaces_latents(on_cpu):
+def test_callback_on_step_end_sees_and_replaces_latents():
     from easyanimate_b200 import EasyAnimatePipeline
-    t, v = _modules(on_cpu)
+    t, v = _modules()
     g = torch.Generator().manual_seed(3)
     lat = torch.randn(1, 16, LF, H // 8, W // 8, generator=g).to(bf16)
     pe, ne = _embeds(g)
@@ -162,9 +147,9 @@ def test_callback_on_step_end_sees_and_replaces_latents(on_cpu):
 
 
 @pytest.mark.parametrize("strength", [1.0, 0.7])
-def test_inpaint_pipeline_equals_the_reference_pipeline(on_cpu, strength):
+def test_inpaint_pipeline_equals_the_reference_pipeline(strength):
     from easyanimate_b200 import EasyAnimateInpaintPipeline
-    t, v = _modules(on_cpu, in_channels=33, seeds=(73, 74), resize_inpaint_mask_directly=True, enable_clip_in_inpaint=False,
+    t, v = _modules(in_channels=33, seeds=(73, 74), resize_inpaint_mask_directly=True, enable_clip_in_inpaint=False,
                     add_noise_in_inpaint_model=True)
     g = torch.Generator().manual_seed(4)
     video = torch.tile(torch.rand(1, 3, 1, H, W, generator=g), [1, 1, FRAMES, 1, 1])
@@ -178,10 +163,10 @@ def test_inpaint_pipeline_equals_the_reference_pipeline(on_cpu, strength):
               lambda: ref_pipeline.reference_inpaint_pipeline(t, v)(generator=torch.Generator().manual_seed(9), **kw).frames)
 
 
-def test_inpaint_pipeline_all_masked_is_zero_conditioning(on_cpu):
+def test_inpaint_pipeline_all_masked_is_zero_conditioning():
     """mask == 255 everywhere: predict_t2v through the InP checkpoint (pipeline_easyanimate_inpaint.py:1322-1336)."""
     from easyanimate_b200 import EasyAnimateInpaintPipeline
-    t, v = _modules(on_cpu, in_channels=33, seeds=(73, 74), resize_inpaint_mask_directly=True, enable_clip_in_inpaint=False)
+    t, v = _modules(in_channels=33, seeds=(73, 74), resize_inpaint_mask_directly=True, enable_clip_in_inpaint=False)
     g = torch.Generator().manual_seed(6)
     video = torch.zeros(1, 3, FRAMES, H, W)
     mask = torch.full((1, 1, FRAMES, H, W), 255.0)
@@ -193,9 +178,9 @@ def test_inpaint_pipeline_all_masked_is_zero_conditioning(on_cpu):
 
 
 @pytest.mark.parametrize("mode", ["control_video+ref", "control_video", "camera", "none"])
-def test_control_pipeline_equals_the_reference_pipeline(on_cpu, mode):
+def test_control_pipeline_equals_the_reference_pipeline(mode):
     from easyanimate_b200 import EasyAnimateControlPipeline
-    t, v = _modules(on_cpu, in_channels=48, seeds=(75, 76), add_ref_latent_in_control_model=True)
+    t, v = _modules(in_channels=48, seeds=(75, 76), add_ref_latent_in_control_model=True)
     g = torch.Generator().manual_seed(8)
     lat = torch.randn(1, 16, LF, H // 8, W // 8, generator=g).to(bf16)
     pe, ne = _embeds(g)
@@ -252,10 +237,10 @@ class _FakeTextEncoder(torch.nn.Module):
         return type("Out", (), {"hidden_states": [h0, h1, self.mix(h1)]})()
 
 
-def test_prompt_strings_go_through_the_llm_branch_like_the_reference(on_cpu):
+def test_prompt_strings_go_through_the_llm_branch_like_the_reference():
     """prompt / negative_prompt as strings: chat template -> tokenizer -> text_encoder(...).hidden_states[-2] -> the loop."""
     from easyanimate_b200 import EasyAnimatePipeline
-    t, v = _modules(on_cpu)
+    t, v = _modules()
     torch.manual_seed(0)
     tok, enc = _FakeTokenizer(), _FakeTextEncoder(128).to(bf16)
     ref = None
@@ -275,11 +260,11 @@ def test_prompt_strings_go_through_the_llm_branch_like_the_reference(on_cpu):
         GOLD.same_sample(f"prompt_embeds_{i}", b, e_ref[i] if LIVE else None)
 
 
-def test_teacache_inside_the_pipeline_call_matches_the_reference_pipeline(on_cpu):
+def test_teacache_inside_the_pipeline_call_matches_the_reference_pipeline():
     """predict_t2v.py:275-278 enables TeaCache on the transformer before calling the pipeline: the skip decisions are taken
     inside `transformer.forward`, so both pipelines see the same cached / computed steps and the same frames."""
     from easyanimate_b200 import EasyAnimatePipeline
-    t, v = _modules(on_cpu)
+    t, v = _modules()
     coeffs = [1.07862322, -4.19362456, 3.06725828, 0.33161686, 0.02374758]
     g = torch.Generator().manual_seed(21)
     lat = torch.randn(1, 16, LF, H // 8, W // 8, generator=g).to(bf16)
@@ -297,10 +282,10 @@ def test_teacache_inside_the_pipeline_call_matches_the_reference_pipeline(on_cpu
     _same_ref("teacache", got, lambda: want)
 
 
-def test_two_videos_per_prompt(on_cpu):
+def test_two_videos_per_prompt():
     """num_images_per_prompt = 2: embeddings repeated, a batch of two latents (drawn at once, or from one generator per sample)."""
     from easyanimate_b200 import EasyAnimatePipeline
-    t, v = _modules(on_cpu)
+    t, v = _modules()
     pe, ne = _embeds(torch.Generator().manual_seed(31))
     kw = dict(video_length=FRAMES, height=H, width=W, num_inference_steps=2, guidance_scale=6.0, num_images_per_prompt=2,
               **_mask_kw(pe, ne))
@@ -312,14 +297,14 @@ def test_two_videos_per_prompt(on_cpu):
         pipe(generator=[torch.Generator().manual_seed(1)] * 3, **kw)
 
 
-def test_load_pipeline_follows_the_predict_scripts_loading_sequence(on_cpu, tmp_path):
+def test_load_pipeline_follows_the_predict_scripts_loading_sequence(tmp_path):
     """predict_t2v.py:94-255 on a released-layout directory (transformer/, vae/, scheduler/ with config.json + safetensors):
     `load_pipeline` returns the pipeline class the scripts pick (InP checkpoint -> inpaint pipeline), with the scheduler of
     scheduler_config.json, and its call equals the call of a pipeline built by hand from the same weights."""
     import json
     from safetensors.torch import save_file
     from easyanimate_b200 import EasyAnimateInpaintPipeline, EasyAnimatePipeline, load_pipeline
-    t, v = _modules(on_cpu, in_channels=33, seeds=(91, 92), resize_inpaint_mask_directly=True, enable_clip_in_inpaint=False)
+    t, v = _modules(in_channels=33, seeds=(91, 92), resize_inpaint_mask_directly=True, enable_clip_in_inpaint=False)
     for name, module in (("transformer", t), ("vae", v)):
         d = tmp_path / name
         d.mkdir()
@@ -345,7 +330,7 @@ def test_load_pipeline_follows_the_predict_scripts_loading_sequence(on_cpu, tmp_
     by_hand = EasyAnimateInpaintPipeline(vae=v, transformer=t, scheduler=FlowMatchEulerDiscreteScheduler(shift=3.0))
     _same(pipe(generator=torch.Generator().manual_seed(94), **kw).frames, by_hand(generator=torch.Generator().manual_seed(94), **kw).frames)
     # a 16-channel checkpoint gives the text-to-video pipeline
-    t16, _ = _modules(on_cpu, seeds=(95, 92))
+    t16, _ = _modules(seeds=(95, 92))
     (tmp_path / "transformer" / "config.json").write_text(json.dumps(dict(t16.config)))
     save_file({k: x.detach().contiguous() for k, x in t16.state_dict().items()},
               str(tmp_path / "transformer" / "diffusion_pytorch_model.safetensors"))
@@ -353,11 +338,11 @@ def test_load_pipeline_follows_the_predict_scripts_loading_sequence(on_cpu, tmp_
 
 
 @pytest.mark.parametrize("video_length,h,w", [(1, 64, 96), (9, 48, 80), (5, 70, 100)])
-def test_t2v_edge_shapes(on_cpu, video_length, h, w):
+def test_t2v_edge_shapes(video_length, h, w):
     """A single image (video_length 1 -> one latent frame), 1 + 8 frames, and a size that is not a multiple of 16 (both pipelines
     round it down: pipeline_easyanimate.py:874-876)."""
     from easyanimate_b200 import EasyAnimatePipeline
-    t, v = _modules(on_cpu)
+    t, v = _modules()
     pe, ne = _embeds(torch.Generator().manual_seed(41))
     kw = dict(video_length=video_length, height=h, width=w, num_inference_steps=2, guidance_scale=6.0, **_mask_kw(pe, ne))
     got = EasyAnimatePipeline(vae=v, transformer=t)(generator=torch.Generator().manual_seed(42), **kw).frames
@@ -366,11 +351,11 @@ def test_t2v_edge_shapes(on_cpu, video_length, h, w):
               lambda: ref_pipeline.reference_pipeline(t, v)(generator=torch.Generator().manual_seed(42), **kw).frames)
 
 
-def test_inpaint_pipeline_with_vae_encoded_mask(on_cpu):
+def test_inpaint_pipeline_with_vae_encoded_mask():
     """resize_inpaint_mask_directly = False (EasyAnimate V5 InP: 16 + 16 + 16 input channels): the mask itself goes through
     `vae.encode` (pipeline_easyanimate_inpaint.py:1364-1376, 781-792) instead of being resized."""
     from easyanimate_b200 import EasyAnimateInpaintPipeline
-    t, v = _modules(on_cpu, in_channels=48, seeds=(77, 78), resize_inpaint_mask_directly=False, enable_clip_in_inpaint=False)
+    t, v = _modules(in_channels=48, seeds=(77, 78), resize_inpaint_mask_directly=False, enable_clip_in_inpaint=False)
     g = torch.Generator().manual_seed(14)
     video = torch.rand(1, 3, FRAMES, H, W, generator=g)
     mask = torch.zeros_like(video[:, :1])
@@ -382,11 +367,11 @@ def test_inpaint_pipeline_with_vae_encoded_mask(on_cpu):
               lambda: ref_pipeline.reference_inpaint_pipeline(t, v)(generator=torch.Generator().manual_seed(15), **kw).frames)
 
 
-def test_inpaint_reference_video_noise_with_sampled_strength(on_cpu):
+def test_inpaint_reference_video_noise_with_sampled_strength():
     """noise_aug_strength = None: one noise level per sample drawn from exp(N(-3, 0.5)) with the GLOBAL generator
     (pipeline_easyanimate_inpaint.py:153-157), then the noise itself with the call's generator."""
     from easyanimate_b200 import EasyAnimateInpaintPipeline
-    t, v = _modules(on_cpu, in_channels=33, seeds=(73, 74), resize_inpaint_mask_directly=True, enable_clip_in_inpaint=False,
+    t, v = _modules(in_channels=33, seeds=(73, 74), resize_inpaint_mask_directly=True, enable_clip_in_inpaint=False,
                     add_noise_in_inpaint_model=True)
     g = torch.Generator().manual_seed(16)
     video = torch.rand(1, 3, FRAMES, H, W, generator=g)

@@ -79,14 +79,7 @@ def test_reference_pipeline_call_pins_the_oracle_loop_bf16():
 def test_reference_pipeline_drives_the_product_modules(monkeypatch):
     from easyanimate_b200.autoencoder_magvit import AutoencoderKLMagvit
     from easyanimate_b200.transformer3d import EasyAnimateTransformer3DModel
-    cpu_ops.install(monkeypatch)
-    cpu_ops.install_vae(monkeypatch)
-
-    def decode_on_cpu(self, z):  # the product refuses CPU latents (no CPU path); the host logic under test starts behind that guard
-        outs = [self._decode_one(zb) for zb in z.to(bf16)]
-        return outs[0] if len(outs) == 1 else torch.cat(outs, dim=0)
-
-    monkeypatch.setattr(AutoencoderKLMagvit, "_decode", decode_on_cpu)
+    cpu_ops.use_stand_ins(monkeypatch)
     lat, pe, ne = (t.to(bf16) for t in _inputs(7))
     ob = dit.init_weights_(dit.OracleTransformer3D(**CFG), 31).to(bf16)
     ours_t = EasyAnimateTransformer3DModel(**CFG, time_position_encoding_type="3d_rope").to(bf16)
@@ -128,9 +121,7 @@ def test_reference_inpaint_pipeline_drives_the_product_modules(monkeypatch):
     import easyanimate_b200.autoencoder_magvit as A
     from easyanimate_b200.transformer3d import EasyAnimateTransformer3DModel
     from oracle import ref_dit, ref_vae
-    cpu_ops.install(monkeypatch)
-    cpu_ops.install_vae(monkeypatch)
-    monkeypatch.setattr(A, "_require_cuda", lambda t, what: None)  # lift the no-CPU-path guard, nothing else
+    cpu_ops.use_stand_ins(monkeypatch)
     video, mask, pe, ne = _i2v_inputs()
     pe, ne = pe.to(bf16), ne.to(bf16)
     ocfg = {k: v for k, v in I2V_CFG.items() if k in CFG}
@@ -173,9 +164,7 @@ def test_reference_control_pipeline_drives_the_product_modules(monkeypatch, with
     import easyanimate_b200.autoencoder_magvit as A
     from easyanimate_b200.transformer3d import EasyAnimateTransformer3DModel
     from oracle import ref_dit, ref_vae
-    cpu_ops.install(monkeypatch)
-    cpu_ops.install_vae(monkeypatch)
-    monkeypatch.setattr(A, "_require_cuda", lambda t, what: None)
+    cpu_ops.use_stand_ins(monkeypatch)
     g = torch.Generator().manual_seed(13)
     lat = torch.randn(1, 16, LF, H // 8, W // 8, generator=g).to(bf16)
     control = torch.rand(1, 3, FRAMES, H, W, generator=g)
@@ -218,7 +207,7 @@ def test_reference_merge_lora_walks_the_product_transformer(monkeypatch):
     fn = [n for n in ast.parse(open(path).read()).body if isinstance(n, ast.FunctionDef) and n.name == "merge_lora"]
     ns = {"torch": torch, "defaultdict": defaultdict, "load_file": None}
     exec(compile(ast.Module(body=fn, type_ignores=[]), path, "exec"), ns)
-    cpu_ops.install(monkeypatch)
+    cpu_ops.use_stand_ins(monkeypatch)
     cfg = dict(CFG, time_position_encoding_type="3d_rope")
     ob = dit.init_weights_(dit.OracleTransformer3D(**CFG), 81).to(bf16)
     ours = EasyAnimateTransformer3DModel(**cfg).to(bf16)

@@ -101,6 +101,9 @@ class AttnArgs(C.Structure):
     ]
 
 
+MAX_E4M3_SEGMENTS = 64
+
+
 class ConvArgs(C.Structure):
     _fields_ = [
         ("x", vp), ("w", vp), ("bias", vp), ("residual", vp), ("out", vp),
@@ -135,6 +138,8 @@ ea_cfg_euler_step = _sig("ea_cfg_euler_step", [vp, vp, vp, vp, i64, f32, i32, f3
 ea_l1_sums = _sig("ea_l1_sums", [vp, vp, vp, i64, vp])
 ea_ew_addsub = _sig("ea_ew_addsub", [vp, vp, vp, i64, i32, vp])
 ea_dequant_e4m3 = _sig("ea_dequant_e4m3", [vp, vp, i64, vp])
+ea_h2d_block = _sig("ea_h2d_block", [vp, vp, i64, vp, vp, vp])
+ea_expand_e4m3_segments = _sig("ea_expand_e4m3_segments", [vp, C.POINTER(i64), C.POINTER(vp), C.POINTER(i64), i32, vp])
 ea_ipc_export = _sig("ea_ipc_export", [vp, vp, C.POINTER(i64)])
 ea_ipc_open = _sig("ea_ipc_open", [vp, C.POINTER(vp)])
 ea_ipc_close = _sig("ea_ipc_close", [vp])

@@ -19,6 +19,25 @@ extern "C" const char* ea_last_error(void) { return ea::last_error_cstr(); }
 extern "C" int ea_abi_version(void) { return 4; }
 extern "C" uint64_t ea_launch_count(void) { return ea::g_launches.load(std::memory_order_relaxed); }
 
+extern "C" int ea_h2d_block(void* dst, const void* src_host, int64_t bytes, void* wait_event, void* done_event,
+                            void* copy_stream) {
+  EA_REQUIRE(dst && src_host && bytes > 0 && done_event, "ea_h2d_block: bad arguments");
+  cudaPointerAttributes attr{};
+  cudaError_t e = cudaPointerGetAttributes(&attr, src_host);
+  if (e != cudaSuccess || attr.type != cudaMemoryTypeHost) {
+    (void)cudaGetLastError();
+    return ea::fail(EA_ERR_INVALID, "ea_h2d_block: the source must be pinned host memory (an unpinned copy would not overlap)");
+  }
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(copy_stream);
+  if (wait_event && (e = cudaStreamWaitEvent(s, reinterpret_cast<cudaEvent_t>(wait_event), 0)) != cudaSuccess)
+    return ea::fail(EA_ERR_CUDA, std::string("ea_h2d_block: cudaStreamWaitEvent: ") + cudaGetErrorString(e));
+  if ((e = cudaMemcpyAsync(dst, src_host, (size_t)bytes, cudaMemcpyHostToDevice, s)) != cudaSuccess)
+    return ea::fail(EA_ERR_CUDA, std::string("ea_h2d_block: cudaMemcpyAsync: ") + cudaGetErrorString(e));
+  if ((e = cudaEventRecord(reinterpret_cast<cudaEvent_t>(done_event), s)) != cudaSuccess)
+    return ea::fail(EA_ERR_CUDA, std::string("ea_h2d_block: cudaEventRecord: ") + cudaGetErrorString(e));
+  return EA_OK;
+}
+
 extern "C" int ea_enable_peer_access(int32_t peer_device) {
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return ea::fail(EA_ERR_CUDA, "ea_enable_peer_access: no current device");

@@ -338,36 +338,79 @@ __global__ void ew_addsub_kernel(const bf16* __restrict__ a, const bf16* __restr
   *reinterpret_cast<uint32_t*>(out + i) = sub ? pack_bf16x2(x.x - y.x, x.y - y.y) : pack_bf16x2(x.x + y.x, x.y + y.y);
 }
 // e4m3fn (1-4-3, bias 7, no infinities, S.1111.111 = NaN) -> bf16, exact: every e4m3 value is a bf16 value.  The 256-entry
-// table is rebuilt per block in shared memory; 16 weights per thread (one 16-byte load, two 16-byte stores).
+// table is rebuilt per block in shared memory (blockDim.x == 256: one entry per thread).
+__device__ __forceinline__ void build_e4m3_lut(uint16_t* lut) {
+  const int v = threadIdx.x;
+  const int sgn = v >> 7, e = (v >> 3) & 15, m = v & 7;
+  float f;
+  if (e == 15 && m == 7) f = __int_as_float(0x7fc00000);
+  else if (e == 0) f = ldexpf((float)m, -9);              // subnormal: m/8 * 2^-6
+  else f = ldexpf(1.0f + (float)m * 0.125f, e - 7);
+  f = sgn ? -f : f;
+  lut[v] = __bfloat16_as_ushort(__float2bfloat16_rn(f));
+}
+
+// 16 weights: one 16-byte load, two 16-byte stores.
+__device__ __forceinline__ void expand_e4m3x16(const uint16_t* lut, const uint8_t* src, bf16* dst) {
+  const uint4 u = *reinterpret_cast<const uint4*>(src);
+  const uint32_t uw[4] = {u.x, u.y, u.z, u.w};
+  uint32_t o[8];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    o[2 * k] = lut[uw[k] & 0xff] | ((uint32_t)lut[(uw[k] >> 8) & 0xff] << 16);
+    o[2 * k + 1] = lut[(uw[k] >> 16) & 0xff] | ((uint32_t)lut[uw[k] >> 24] << 16);
+  }
+  uint4* d = reinterpret_cast<uint4*>(dst);
+  d[0] = make_uint4(o[0], o[1], o[2], o[3]);
+  d[1] = make_uint4(o[4], o[5], o[6], o[7]);
+}
+
 __global__ void dequant_e4m3_kernel(const uint8_t* __restrict__ w8, bf16* __restrict__ w16, int64_t n) {
   __shared__ uint16_t lut[256];
-  {
-    const int v = threadIdx.x;  // blockDim.x == 256
-    const int sgn = v >> 7, e = (v >> 3) & 15, m = v & 7;
-    float f;
-    if (e == 15 && m == 7) f = __int_as_float(0x7fc00000);
-    else if (e == 0) f = ldexpf((float)m, -9);              // subnormal: m/8 * 2^-6
-    else f = ldexpf(1.0f + (float)m * 0.125f, e - 7);
-    f = sgn ? -f : f;
-    lut[v] = __bfloat16_as_ushort(__float2bfloat16_rn(f));
-  }
+  build_e4m3_lut(lut);
   __syncthreads();
   const int64_t i0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * 16;
   if (i0 >= n) return;
   if (i0 + 16 <= n) {
-    const uint4 u = *reinterpret_cast<const uint4*>(w8 + i0);
-    const uint32_t uw[4] = {u.x, u.y, u.z, u.w};
-    uint32_t o[8];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      o[2 * k] = lut[uw[k] & 0xff] | ((uint32_t)lut[(uw[k] >> 8) & 0xff] << 16);
-      o[2 * k + 1] = lut[(uw[k] >> 16) & 0xff] | ((uint32_t)lut[uw[k] >> 24] << 16);
-    }
-    uint4* dst = reinterpret_cast<uint4*>(w16 + i0);
-    dst[0] = make_uint4(o[0], o[1], o[2], o[3]);
-    dst[1] = make_uint4(o[4], o[5], o[6], o[7]);
+    expand_e4m3x16(lut, w8 + i0, w16 + i0);
   } else {
     for (int64_t i = i0; i < n; ++i) w16[i] = __ushort_as_bfloat16(lut[w8[i]]);
+  }
+}
+
+// A whole packed block in one launch: segment s expands n[s] weights from src + src_off[s] into dst[s].  first_vec[s] is the
+// index of the segment's first 16-weight vector in the launch (prefix sums, first_vec[count] = total); a grid-stride loop
+// walks the vectors and finds each one's segment by binary search in the parameter table.
+struct E4m3Segments {
+  const uint8_t* src;
+  int64_t src_off[EA_MAX_E4M3_SEGMENTS];
+  bf16* dst[EA_MAX_E4M3_SEGMENTS];
+  int64_t n[EA_MAX_E4M3_SEGMENTS];
+  int64_t first_vec[EA_MAX_E4M3_SEGMENTS + 1];
+  int count;
+};
+
+__global__ void __launch_bounds__(256) expand_e4m3_segments_kernel(const __grid_constant__ E4m3Segments t) {
+  __shared__ uint16_t lut[256];
+  build_e4m3_lut(lut);
+  __syncthreads();
+  const int64_t total = t.first_vec[t.count];
+  for (int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; v < total; v += (int64_t)gridDim.x * blockDim.x) {
+    int lo = 0, hi = t.count - 1;  // last segment with first_vec <= v
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (t.first_vec[mid] <= v) lo = mid;
+      else hi = mid - 1;
+    }
+    const int64_t i0 = (v - t.first_vec[lo]) * 16;
+    const uint8_t* src = t.src + t.src_off[lo] + i0;
+    bf16* dst = t.dst[lo] + i0;
+    const int64_t left = t.n[lo] - i0;
+    if (left >= 16) {
+      expand_e4m3x16(lut, src, dst);
+    } else {
+      for (int64_t i = 0; i < left; ++i) dst[i] = __ushort_as_bfloat16(lut[src[i]]);
+    }
   }
 }
 
@@ -481,6 +524,30 @@ extern "C" int ea_dequant_e4m3(const void* w8, void* w16, int64_t n, void* strea
              "ea_dequant_e4m3: pointers must be 16-byte aligned");
   return launch(dequant_e4m3_kernel, grid_1d((n + 15) / 16, 256), 256, 0, stream, "dequant_e4m3_kernel",
                 (const uint8_t*)w8, (bf16*)w16, n);
+}
+
+extern "C" int ea_expand_e4m3_segments(const void* src, const int64_t* src_offsets, void* const* dsts, const int64_t* counts,
+                                       int32_t n_segs, void* stream) {
+  EA_REQUIRE(src && src_offsets && dsts && counts, "ea_expand_e4m3_segments: null pointer");
+  EA_REQUIRE(n_segs > 0 && n_segs <= EA_MAX_E4M3_SEGMENTS, "ea_expand_e4m3_segments: 1 to EA_MAX_E4M3_SEGMENTS segments");
+  EA_REQUIRE((reinterpret_cast<uintptr_t>(src) & 15) == 0, "ea_expand_e4m3_segments: src must be 16-byte aligned");
+  E4m3Segments t{};
+  t.src = (const uint8_t*)src;
+  t.count = n_segs;
+  int64_t vecs = 0;
+  for (int s = 0; s < n_segs; ++s) {
+    EA_REQUIRE(dsts[s] && counts[s] > 0 && src_offsets[s] >= 0, "ea_expand_e4m3_segments: bad segment");
+    EA_REQUIRE(src_offsets[s] % 16 == 0 && (reinterpret_cast<uintptr_t>(dsts[s]) & 15) == 0,
+               "ea_expand_e4m3_segments: segment offsets and destinations must be 16-byte aligned");
+    t.src_off[s] = src_offsets[s];
+    t.dst[s] = (bf16*)dsts[s];
+    t.n[s] = counts[s];
+    t.first_vec[s] = vecs;
+    vecs += (counts[s] + 15) / 16;
+  }
+  t.first_vec[n_segs] = vecs;
+  const unsigned blocks = std::min(grid_1d(vecs, 256), 8u * sm_count());
+  return launch(expand_e4m3_segments_kernel, blocks, 256, 0, stream, "expand_e4m3_segments_kernel", t);
 }
 
 extern "C" int ea_l1_sums(const void* cur, const void* prev, void* sums, int64_t n, void* stream) {

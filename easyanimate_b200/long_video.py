@@ -143,7 +143,8 @@ def generate_long_video(pipe, prompt=None, *, video_length: int, partial_video_l
         latents = pipe.denoise_to_latents(prompt, video_length=n, video=video, mask_video=mask, height=height, width=width,
                                           num_inference_steps=num_inference_steps, guidance_scale=guidance_scale,
                                           generator=generator, negative_prompt=negative_prompt, strength=1, **pipe_kwargs)
-        frames = vae.decode_scaled_video(latents).contiguous()
+        with pipe._on_device("vae"):  # model CPU offload: the VAE visits the GPU for the decode only
+            frames = vae.decode_scaled_video(latents).contiguous()
         if tuple(frames.shape) != (1, 3, n, height, width):
             raise ValueError(f"window {k} decoded to {list(frames.shape)}, expected [1, 3, {n}, {height}, {width}]")
         vae_ops.frames_out_blend(frames, out[:, :, t0:t0 + n], ov if k else 0)

@@ -223,6 +223,40 @@ def dequant_e4m3(w8: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
     return out
 
 
+def e4m3_segment_table(segments) -> tuple:
+    """[(byte offset in the packed source, bf16 CUDA destination tensor)] -> the ctypes table expand_e4m3_segments takes.
+    Build it once per (slot, staging block) pair: the destinations' addresses are baked in."""
+    if not 0 < len(segments) <= L.MAX_E4M3_SEGMENTS:
+        raise L.EaError(f"expand_e4m3_segments takes 1 to {L.MAX_E4M3_SEGMENTS} segments, got {len(segments)}")
+    n = len(segments)
+    offs, dsts, counts = (L.i64 * n)(), (L.vp * n)(), (L.i64 * n)()
+    for i, (off, dst) in enumerate(segments):
+        _req(dst, name="segment destination")
+        assert dst.is_contiguous()
+        offs[i], dsts[i], counts[i] = off, dst.data_ptr(), dst.numel()
+    return offs, dsts, counts, n
+
+
+def expand_e4m3_segments(src: torch.Tensor, table) -> None:
+    """Expand a packed e4m3 block (a uint8 / float8_e4m3fn CUDA buffer) into bf16 destinations in one launch; `table` from
+    e4m3_segment_table.  Bit-identical to one dequant_e4m3 per segment."""
+    if not src.is_cuda or src.dtype not in (torch.uint8, torch.float8_e4m3fn):
+        raise L.EaError(f"expand_e4m3_segments takes a CUDA uint8 / float8_e4m3fn buffer, got {src.dtype} on {src.device}")
+    offs, dsts, counts, n = table
+    L.check(L.ea_expand_e4m3_segments(_p(src), offs, dsts, counts, n, _stream()), "ea_expand_e4m3_segments")
+
+
+def h2d_block(dst: torch.Tensor, src: torch.Tensor, wait_event: Optional[torch.cuda.Event], done_event: torch.cuda.Event,
+              copy_stream: torch.cuda.Stream) -> None:
+    """Enqueue on copy_stream: wait for wait_event, copy the pinned host buffer src into the device slot dst (its first
+    src.nbytes bytes), record done_event."""
+    if not dst.is_cuda or src.is_cuda or not src.is_pinned():
+        raise L.EaError("h2d_block copies a pinned host buffer into a CUDA buffer")
+    assert src.is_contiguous() and dst.is_contiguous() and src.nbytes <= dst.nbytes
+    L.check(L.ea_h2d_block(_p(dst), _p(src), src.nbytes, None if wait_event is None else wait_event.cuda_event,
+                           done_event.cuda_event, copy_stream.cuda_stream), "ea_h2d_block")
+
+
 def ew_add(a: torch.Tensor, b: torch.Tensor, out: Optional[torch.Tensor] = None, subtract: bool = False) -> torch.Tensor:
     _req(a, name="a"); _req(b, name="b")
     assert a.shape == b.shape and a.is_contiguous() and b.is_contiguous()

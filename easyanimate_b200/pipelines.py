@@ -18,6 +18,7 @@ the CLIP-image branch of the inpaint pipeline (V5.1: `enable_clip_in_inpaint: fa
 16-channel transformer, the Bert/T5 tokenizer branch of V5 (`text_embed_dim_t5`), non flow-matching schedulers, ComfyUI's bar."""
 from __future__ import annotations
 
+from contextlib import contextmanager
 from dataclasses import dataclass
 from typing import Callable, Dict, List, Optional, Tuple, Union
 
@@ -107,6 +108,57 @@ class _NativePipelineBase:
         self.vae_scale_factor = 2 ** (len(self.vae.config.block_out_channels) - 1)
         self.cfg_group = cfg_group
         self._guidance_scale, self._guidance_rescale, self._num_timesteps, self._interrupt = 1.0, 0.0, 0, False
+        self._offload_device = None  # the GPU of the offload modes (enable_model_cpu_offload / enable_sequential_cpu_offload)
+        self._model_offload = ()  # names of the modules that live in host memory and visit the GPU while they are used
+
+    # ---- the reference drivers' GPU_memory_mode (predict_t2v.py:26-37,256-273) ----------------------------------
+    def enable_model_cpu_offload(self, device="cuda"):
+        """Every module lives in host memory and moves to `device` only while it is used: the text encoder for prompt
+        encoding, the VAE for encode / decode, the transformer for the denoise loop; each goes back before the next comes up.
+        Frames are those of the resident pipeline."""
+        self._offload_device = torch.device(device)
+        self._model_offload = ("text_encoder", "text_encoder_2", "vae", "transformer")
+        for name in self._model_offload:
+            self._to_host(getattr(self, name))
+        return self
+
+    def enable_sequential_cpu_offload(self, device="cuda"):
+        """The transformer streams its blocks from pinned host memory (EasyAnimateTransformer3DModel.
+        enable_sequential_cpu_offload), the text encoder is offloaded per model as in enable_model_cpu_offload, and the VAE
+        stays on `device`: it is small - the state dict of the V5.1-shaped AutoencoderKLMagvit holds 246.5 M values, 0.49 GB in bf16 -
+        next to the activations of its decode."""
+        self._offload_device = torch.device(device)
+        self._model_offload = ("text_encoder", "text_encoder_2")
+        for name in self._model_offload:
+            self._to_host(getattr(self, name))
+        self.vae.to(self._offload_device)
+        self.transformer.enable_sequential_cpu_offload(self._offload_device)
+        return self
+
+    @staticmethod
+    def _to_host(module):
+        """Module to host memory, its device-side derived copies dropped, and the freed device memory handed back to the
+        driver (torch's caching allocator would otherwise keep it reserved for this process only)."""
+        if module is not None:
+            was_on_gpu = any(p.is_cuda for p in module.parameters())
+            module.to("cpu")
+            if hasattr(module, "invalidate_weight_caches"):  # device copies derived from the parameters (fused q/k/v, ...)
+                module.invalidate_weight_caches()
+            if was_on_gpu:
+                torch.cuda.empty_cache()
+
+    @contextmanager
+    def _on_device(self, name):
+        """Module `name` on the execution device for the duration of the block (model offload), else as it is."""
+        module = getattr(self, name)
+        if module is None or name not in self._model_offload:
+            yield module
+            return
+        module.to(self._offload_device)
+        try:
+            yield module
+        finally:
+            self._to_host(module)
 
     # ---- the reference pipelines' read-only properties
     @property
@@ -131,6 +183,8 @@ class _NativePipelineBase:
 
     @property
     def _execution_device(self):
+        if self._offload_device is not None:
+            return self._offload_device
         return next(self.transformer.parameters()).device
 
     @property
@@ -163,11 +217,12 @@ class _NativePipelineBase:
         text = self.tokenizer.apply_chat_template(messages, tokenize=False, add_generation_prompt=True)
         tok = self.tokenizer(text=[text], padding="max_length", max_length=max_length, truncation=True,
                              return_attention_mask=True, padding_side="right", return_tensors="pt")
-        tok = tok.to(self.text_encoder.device)
         if not self.transformer.config.enable_text_attention_mask:
             raise ValueError("LLM needs attention_mask")
-        hidden = self.text_encoder(input_ids=tok.input_ids, attention_mask=tok.attention_mask,
-                                   output_hidden_states=True).hidden_states[-2]
+        with self._on_device("text_encoder") as text_encoder:
+            tok = tok.to(text_encoder.device)
+            hidden = text_encoder(input_ids=tok.input_ids, attention_mask=tok.attention_mask,
+                                  output_hidden_states=True).hidden_states[-2]
         return hidden, tok.attention_mask
 
     def encode_prompt(self, prompt, device, dtype, num_images_per_prompt=1, do_classifier_free_guidance=True, negative_prompt=None,
@@ -256,7 +311,8 @@ class _NativePipelineBase:
     def _encode_to_latents(self, pixels: torch.Tensor, device, dtype) -> torch.Tensor:
         """`vae.encode(x)[0].mode() * scaling_factor`, one sample at a time (pipeline_easyanimate_inpaint.py:800-812)."""
         pixels = pixels.to(device=device, dtype=dtype)
-        out = [self.vae.encode(pixels[i:i + 1])[0].mode() for i in range(pixels.shape[0])]
+        with self._on_device("vae") as vae:
+            out = [vae.encode(pixels[i:i + 1])[0].mode() for i in range(pixels.shape[0])]
         return torch.cat(out, dim=0) * self.vae.config.scaling_factor
 
     @staticmethod
@@ -284,6 +340,13 @@ class _NativePipelineBase:
     # ---- the loop + decode ---------------------------------------------------------------------------------------
     def _denoise(self, latents, prompt_embeds, negative_prompt_embeds, height, width, first_index, num_steps, guidance_scale,
                  inpaint_latents=None, control_latents=None, callback_on_step_end=None, callback_tensor_inputs=("latents",)):
+        with self._on_device("transformer"):
+            return self._denoise_resident(latents, prompt_embeds, negative_prompt_embeds, height, width, first_index, num_steps,
+                                          guidance_scale, inpaint_latents, control_latents, callback_on_step_end,
+                                          callback_tensor_inputs)
+
+    def _denoise_resident(self, latents, prompt_embeds, negative_prompt_embeds, height, width, first_index, num_steps,
+                          guidance_scale, inpaint_latents, control_latents, callback_on_step_end, callback_tensor_inputs):
         device = latents.device
         sampler = EasyAnimateSampler(self.transformer, vae=self.vae, scheduler=self.scheduler, guidance_scale=guidance_scale,
                                      cfg_group=self.cfg_group)
@@ -313,8 +376,9 @@ class _NativePipelineBase:
     def decode_latents(self, latents: torch.Tensor) -> np.ndarray:
         """pipeline_easyanimate.py:722-742: numpy float32 [B,3,F,H,W] in [0,1] (a view of the pinned host buffer the output
         kernel wrote)."""
-        sampler = EasyAnimateSampler(self.transformer, vae=self.vae, scheduler=self.scheduler)
-        return sampler.decode_latents(latents).numpy()
+        with self._on_device("vae"):
+            sampler = EasyAnimateSampler(self.transformer, vae=self.vae, scheduler=self.scheduler)
+            return sampler.decode_latents(latents).numpy()
 
     def _finish(self, latents, output_type, return_dict):
         video = self.decode_latents(latents)
@@ -559,9 +623,47 @@ class EasyAnimateControlPipeline(_NativePipelineBase):
         return self._finish(latents, output_type, return_dict)
 
 
+GPU_MEMORY_MODES = ("model_full_load", "model_cpu_offload", "model_cpu_offload_and_qfloat8", "sequential_cpu_offload")
+
+
+def store_text_encoder_e4m3(text_encoder: torch.nn.Module, compute_dtype=bf16, keep: str = "embed_tokens") -> torch.nn.Module:
+    """The reference's `sequential_cpu_offload` text encoder (predict_t2v.py:256-265, utils/fp8_optimization.py): every
+    parameter whose name does not contain `keep` is stored as float8_e4m3fn, and every module that has a `weight` (but the
+    root and the `keep` modules) is cast to `compute_dtype` around its own forward, its positional inputs too, and back to
+    e4m3 afterwards.  The prompt embeddings are then the reference's, which differ from those of the bf16 encoder."""
+    e4m3 = torch.float8_e4m3fn
+    for mname, module in text_encoder.named_modules():
+        if keep in mname:
+            continue
+        for pname, p in module.named_parameters():
+            if keep not in pname and p.dtype != e4m3:
+                p.data = p.data.to(e4m3)
+
+    def to_compute(module, args):
+        module._stored_dtype = module.weight.dtype
+        module.to(compute_dtype)
+        return tuple(a.to(compute_dtype) if torch.is_tensor(a) else a for a in args)
+
+    def to_storage(module, args, out):
+        module.to(module._stored_dtype)
+
+    for mname, module in text_encoder.named_modules():
+        if mname and keep not in mname and hasattr(module, "weight"):
+            module.register_forward_pre_hook(to_compute)
+            module.register_forward_hook(to_storage)
+    return text_encoder
+
+
+def _drop_visual_tower(text_encoder) -> None:
+    """predict_t2v.py:260-261,268-270 `del text_encoder.visual`: prompts never reach Qwen2-VL's vision tower."""
+    for owner in (text_encoder, getattr(text_encoder, "model", None)):
+        if owner is not None and "visual" in owner._modules:
+            del owner._modules["visual"]
+
+
 def load_pipeline(model_name: str, config: Union[str, dict, None] = None, weight_dtype=bf16, device="cuda",
                   transformer_path: Optional[str] = None, vae_path: Optional[str] = None, load_text_encoder: bool = True,
-                  cfg_group=None):
+                  cfg_group=None, GPU_memory_mode: str = "model_full_load"):
     """The loading sequence of predict_t2v.py:94-255 / predict_i2v.py for a released EasyAnimateV5.1 directory
     (`transformer/`, `vae/`, `scheduler/`, `tokenizer/`, `text_encoder/`), ending in the pipeline object those scripts build:
     `EasyAnimateInpaintPipeline` when the transformer has more input channels than the VAE has latent channels (the InP /
@@ -571,9 +673,17 @@ def load_pipeline(model_name: str, config: Union[str, dict, None] = None, weight
     `transformer_additional_kwargs` / `vae_kwargs` / `text_encoder_kwargs`; None = the V5.1 values.
     transformer_path / vae_path: optional fine-tuned weights loaded over the released ones (non-strict, like the scripts).
     load_text_encoder: the Qwen2-VL tokenizer and text encoder through `transformers` when their folders exist; without them
-    the pipeline takes `prompt_embeds` (+ masks) instead of prompt strings."""
+    the pipeline takes `prompt_embeds` (+ masks) instead of prompt strings.
+    GPU_memory_mode: the reference drivers' setting (predict_t2v.py:26-37,256-273).  "model_full_load" keeps every module on
+    `device`; "model_cpu_offload" keeps them in host memory and moves each to `device` while it is used
+    (enable_model_cpu_offload); "model_cpu_offload_and_qfloat8" does the same with the transformer stored as float8_e4m3fn
+    and the text encoder's vision tower dropped; "sequential_cpu_offload" streams the transformer's blocks from pinned host
+    memory (enable_sequential_cpu_offload) and stores the text encoder as e4m3 like the reference (store_text_encoder_e4m3)."""
     import os
 
+    if GPU_memory_mode not in GPU_MEMORY_MODES:
+        raise ValueError(f"GPU_memory_mode must be one of {GPU_MEMORY_MODES}, got {GPU_memory_mode!r}")
+    full = GPU_memory_mode == "model_full_load"
     from .autoencoder_magvit import AutoencoderKLMagvit
     from .transformer3d import EasyAnimateTransformer3DModel
 
@@ -607,8 +717,9 @@ def load_pipeline(model_name: str, config: Union[str, dict, None] = None, weight
         state = state["state_dict"] if "state_dict" in state else state
         return module.load_state_dict(state, strict=False)
 
+    t_dtype = torch.float8_e4m3fn if GPU_memory_mode == "model_cpu_offload_and_qfloat8" else weight_dtype  # predict_t2v.py:106
     transformer = EasyAnimateTransformer3DModel.from_pretrained_2d(model_name, subfolder="transformer",
-                                                                   transformer_additional_kwargs=tkw, torch_dtype=weight_dtype,
+                                                                   transformer_additional_kwargs=tkw, torch_dtype=t_dtype,
                                                                    low_cpu_mem_usage=True)
     if transformer_path is not None:
         overlay(transformer, transformer_path)
@@ -621,9 +732,21 @@ def load_pipeline(model_name: str, config: Union[str, dict, None] = None, weight
         from transformers import Qwen2Tokenizer, Qwen2VLForConditionalGeneration
         tokenizer = Qwen2Tokenizer.from_pretrained(os.path.join(model_name, "tokenizer"))
         text_encoder = Qwen2VLForConditionalGeneration.from_pretrained(os.path.join(model_name, "text_encoder"),
-                                                                       torch_dtype=weight_dtype).to(device)
+                                                                       torch_dtype=weight_dtype)
+        if full:
+            text_encoder = text_encoder.to(device)
+        if GPU_memory_mode in ("model_cpu_offload_and_qfloat8", "sequential_cpu_offload"):
+            _drop_visual_tower(text_encoder)
+        if GPU_memory_mode == "sequential_cpu_offload":
+            store_text_encoder_e4m3(text_encoder, weight_dtype)
     scheduler = (FlowMatchEulerDiscreteScheduler.from_pretrained(model_name, subfolder="scheduler")
                  if os.path.isfile(os.path.join(model_name, "scheduler", "scheduler_config.json")) else FlowMatchEulerDiscreteScheduler())
     kind = EasyAnimateInpaintPipeline if transformer.config.in_channels != vae.config.latent_channels else EasyAnimatePipeline
-    return kind(vae=vae.to(device), transformer=transformer.to(device), scheduler=scheduler, tokenizer=tokenizer,
-                text_encoder=text_encoder, cfg_group=cfg_group)
+    if full:
+        return kind(vae=vae.to(device), transformer=transformer.to(device), scheduler=scheduler, tokenizer=tokenizer,
+                    text_encoder=text_encoder, cfg_group=cfg_group)
+    pipe = kind(vae=vae, transformer=transformer, scheduler=scheduler, tokenizer=tokenizer, text_encoder=text_encoder,
+                cfg_group=cfg_group)
+    if GPU_memory_mode == "sequential_cpu_offload":
+        return pipe.enable_sequential_cpu_offload(device)
+    return pipe.enable_model_cpu_offload(device)

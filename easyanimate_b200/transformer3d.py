@@ -259,18 +259,20 @@ class _Fp8Staging:
         """Expand blk8's e4m3 parameters into the staging block (stream-ordered: the previous block's kernels that read the
         staging buffers are ahead of these writes on the same stream) and return it."""
         st = self._staging_block(blk8.attn2 is not None)
-        dst = dict(st.named_parameters())
-        d = st.dim
         for name, p8 in blk8.named_parameters():
-            parts = name.split(".")
-            if parts[0] in ("attn1", "attn2") and parts[1] in ("to_q", "to_k", "to_v"):
-                w, b = getattr(st, parts[0])._fused_static  # q/k/v go straight into the fused projection operand
-                i = ("to_q", "to_k", "to_v").index(parts[1])
-                out = w[i * d:(i + 1) * d] if parts[2] == "weight" else b[i * d:(i + 1) * d]
-            else:
-                out = dst[name].detach()
-            ops.dequant_e4m3(p8.detach().contiguous(), out)
+            ops.dequant_e4m3(p8.detach().contiguous(), self.destination(st, name))
         return st
+
+    @staticmethod
+    def destination(st: "EasyAnimateDiTBlock", name: str) -> torch.Tensor:
+        """Where the staging block `st` holds parameter `name` in bf16: q/k/v go straight into the fused projection operand."""
+        parts = name.split(".")
+        if parts[0] in ("attn1", "attn2") and parts[1] in ("to_q", "to_k", "to_v"):
+            w, b = getattr(st, parts[0])._fused_static
+            d = st.dim
+            i = ("to_q", "to_k", "to_v").index(parts[1])
+            return w[i * d:(i + 1) * d] if parts[2] == "weight" else b[i * d:(i + 1) * d]
+        return st.get_parameter(name).detach()
 
 
 class _Workspace:
@@ -376,6 +378,7 @@ class EasyAnimateTransformer3DModel(nn.Module, ConfigMixinLite):
         self._proj_w_cache: Dict[str, tuple] = {}
         self._ref_pos_cache: Optional[tuple] = None
         self._fp8: Optional[tuple] = None  # (parameter key, _Fp8Staging) when the parameters are stored as float8_e4m3fn
+        self._offload = None  # offload.SequentialOffload, see enable_sequential_cpu_offload
 
     # ----------------------------------------------------------------------------------------------------------
     def enable_teacache(self, num_steps: int, rel_l1_thresh: float,
@@ -402,6 +405,20 @@ class EasyAnimateTransformer3DModel(nn.Module, ConfigMixinLite):
         additive pieces are summed over `group` so that both ranks take the reference's decision."""
         self.cfg_parallel_group = group
 
+    def enable_sequential_cpu_offload(self, device="cuda", streamer=None):
+        """The reference's `sequential_cpu_offload` for this module: the non-block parameters move to `device`, each block's
+        parameters into one pinned host buffer (in the dtype they are stored in: bf16, or float8_e4m3fn), and every forward
+        streams the blocks through two device slots, copying block i+1 on a side stream while block i runs (offload.py).
+        Results are bit-identical to resident execution.  Device memory for parameters: the non-block ones, two slots of one
+        block each, and for e4m3 storage one bf16 staging block.  `.to(...)`, `load_state_dict` and invalidate_weight_caches()
+        are followed: the blocks are repacked on the next forward when their parameters were replaced.  `streamer` replaces
+        the CUDA copy stream and events (tests).  A forward of an offloaded module cannot be captured in a CUDA graph."""
+        from .offload import SequentialOffload
+        self._offload = None
+        self.invalidate_weight_caches()  # device copies a resident forward derived from the blocks (fused q/k/v, ...)
+        self._offload = SequentialOffload(self, device, streamer)
+        return self
+
     def _set_gradient_checkpointing(self, module, value=False):
         self.gradient_checkpointing = value
 
@@ -417,6 +434,8 @@ class EasyAnimateTransformer3DModel(nn.Module, ConfigMixinLite):
         self._proj_w_cache.clear()
         self._ref_pos_cache = None
         self._fp8 = None
+        if self._offload is not None:
+            self._offload.invalidate()
 
     def _fp8_staging(self) -> _Fp8Staging:
         key = ops.param_key(self.proj.weight, self.proj_out.weight)
@@ -484,6 +503,9 @@ class EasyAnimateTransformer3DModel(nn.Module, ConfigMixinLite):
         if self.dtype != bf16 and not fp8:
             raise L.EaError("easyanimate_b200 computes in bf16: call .to(torch.bfloat16) on the module first (or store the "
                             "weights as torch.float8_e4m3fn: they are expanded to bf16 block by block)")
+        off = self._offload
+        if off is not None:
+            off.start()  # before the staging: it puts the non-block parameters back on the device if they were moved
         staging = self._fp8_staging() if fp8 else None
         P = staging.head if fp8 else self  # owner of the non-block parameters the kernels read
         if timestep_cond is not None:
@@ -557,7 +579,10 @@ class EasyAnimateTransformer3DModel(nn.Module, ConfigMixinLite):
         tc = self.teacache
         should_calc = True
         if tc is not None:
-            blk0 = staging.block(self.transformer_blocks[0]) if fp8 else self.transformer_blocks[0]
+            if off is not None:
+                blk0 = off.block(0, staging)
+            else:
+                blk0 = staging.block(self.transformer_blocks[0]) if fp8 else self.transformer_blocks[0]
             mod0 = ops.skinny_linear(temb, blk0.norm1.linear.weight, blk0.norm1.linear.bias, act_in=1)
             modulated = EasyAnimateDiTBlock._ln_mod(x_v, blk0.norm1, mod0, 0, S_v)
             if tc.cnt == 0 or tc.cnt == tc.num_steps - 1:
@@ -590,8 +615,12 @@ class EasyAnimateTransformer3DModel(nn.Module, ConfigMixinLite):
         else:
             ori = x_v.clone() if tc is not None else None  # (device copy; the blocks update x_v in place)
             ws = _Workspace(B, S_v, S_t, d, self.num_heads, ff_inner, dev, sp=sp)
-            for block in self.transformer_blocks:
-                x_v, x_t = (staging.block(block) if fp8 else block)(x_v, x_t, temb, rope, ws)
+            for i, block in enumerate(self.transformer_blocks):
+                if off is not None:
+                    x_v, x_t = off.block(i, staging)(x_v, x_t, temb, rope, ws)
+                    off.release(i)
+                else:
+                    x_v, x_t = (staging.block(block) if fp8 else block)(x_v, x_t, temb, rope, ws)
 
             # 5. final norms + projection (transformer3d.py:1673-1680): norm_final is row-wise, so the text rows that
             #    the reference concatenates and then drops never need to be computed.

@@ -194,6 +194,21 @@ int ea_ew_addsub(const void* a, const void* b, void* out, int64_t n, int32_t sub
  * right before the kernels that consume them.  n elements; both pointers 16-byte aligned. */
 int ea_dequant_e4m3(const void* w8, void* w16, int64_t n, void* stream);
 
+/* Sequential CPU offload (the reference's `sequential_cpu_offload` GPU_memory_mode, predict_t2v.py:256-265): the MMDiT's
+ * blocks live packed in pinned host memory and are streamed through a ring of device slots while the previous block computes.
+ *
+ * ea_h2d_block enqueues on `copy_stream`: wait for `wait_event` (recorded by the caller on the compute stream after the
+ * slot's previous reader; NULL = none), copy `bytes` from the PINNED host buffer `src_host` into the device slot `dst`, record
+ * `done_event` (the compute stream waits on it before reading the slot).  Events are cudaEvent_t created by the caller. */
+int ea_h2d_block(void* dst, const void* src_host, int64_t bytes, void* wait_event, void* done_event, void* copy_stream);
+
+/* One launch expands a packed e4m3 block slot into its bf16 staging parameters: segment s turns counts[s] weights at
+ * src + src_offsets[s] (bytes) into bf16 at dsts[s], bit-identical to ea_dequant_e4m3.  The three segment arrays are HOST
+ * arrays of n_segs <= EA_MAX_E4M3_SEGMENTS entries, read during the call; src, every offset and every dst 16-byte aligned. */
+#define EA_MAX_E4M3_SEGMENTS 64
+int ea_expand_e4m3_segments(const void* src, const int64_t* src_offsets, void* const* dsts, const int64_t* counts,
+                            int32_t n_segs, void* stream);
+
 /* Joint text+video self-attention, non-causal, no mask, head_dim 64:  O = softmax(Q K^T * scale) V.
  * Replaces F.scaled_dot_product_attention + transpose/reshape/split at processor.py:287-303.
  * q,k,v: [B,H,S,64] bf16 contiguous.  Output is token-major and split at S_text:

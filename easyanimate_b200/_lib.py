@@ -102,6 +102,8 @@ class AttnArgs(C.Structure):
 
 
 MAX_E4M3_SEGMENTS = 64
+LORA_W_BF16, LORA_W_E4M3 = 0, 1
+LORA_C_BF16, LORA_C_F32 = 0, 1
 
 
 class ConvArgs(C.Structure):
@@ -140,6 +142,7 @@ ea_ew_addsub = _sig("ea_ew_addsub", [vp, vp, vp, i64, i32, vp])
 ea_dequant_e4m3 = _sig("ea_dequant_e4m3", [vp, vp, i64, vp])
 ea_h2d_block = _sig("ea_h2d_block", [vp, vp, i64, vp, vp, vp])
 ea_expand_e4m3_segments = _sig("ea_expand_e4m3_segments", [vp, C.POINTER(i64), C.POINTER(vp), C.POINTER(i64), i32, vp])
+ea_lora_merge = _sig("ea_lora_merge", [vp, vp, vp, i64, i64, i64, i64, i64, i64, f32, i32, i32, vp])
 ea_ipc_export = _sig("ea_ipc_export", [vp, vp, C.POINTER(i64)])
 ea_ipc_open = _sig("ea_ipc_open", [vp, C.POINTER(vp)])
 ea_ipc_close = _sig("ea_ipc_close", [vp])

@@ -179,6 +179,34 @@ class SequentialOffload:
         if changed:
             self._device_side = None
 
+    def packed_block(self, i: int) -> bool:
+        """Whether block i's parameters are still the views of its packed buffer (no sync() needed since they were replaced)."""
+        pk = self.packs[i] if i < len(self.packs) else None
+        return pk is not None and pk.block_key(self.model.transformer_blocks[i]) == pk.key
+
+    def edit_blocks(self, blocks, fn):
+        """Edit packed blocks in place on the device (a LoRA merge): each block i of `blocks` is copied from its pinned buffer
+        into one device scratch block, fn(i, {parameter name: view of the scratch}) enqueues its kernels on the current stream,
+        and the scratch is copied back into the same buffer.  Parameters, PackedBlocks and host addresses stay as they are, so
+        nothing is repacked.  Returns after the last copy back has landed."""
+        blocks = sorted(set(blocks))
+        if not blocks:
+            return
+        for i in blocks:
+            if not self.packed_block(i):
+                raise L.EaError(f"edit_blocks: block {i} is not packed (its parameters were replaced since the last forward)")
+        self.streamer.drain()  # no slot copy still reads a buffer that is about to be rewritten
+        scratch = torch.empty((max(self.packs[i].host.nbytes for i in blocks),), dtype=torch.uint8, device=self.device)
+        for i in blocks:
+            host = self.packs[i].host
+            dev = scratch[:host.nbytes]
+            dev.copy_(host, non_blocking=True)
+            fn(i, _views(dev, self.packs[i].layout))
+            host.copy_(dev, non_blocking=True)
+        if self.device.type == "cuda":
+            torch.cuda.current_stream(self.device).synchronize()
+        self._device_side = None
+
     # -- device side ----------------------------------------------------------------------------------------------
     def _kind(self, i: int) -> bool:
         return self.model.transformer_blocks[i].attn2 is not None

@@ -223,6 +223,30 @@ def dequant_e4m3(w8: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
     return out
 
 
+def lora_merge(w: torch.Tensor, up: torch.Tensor, down: torch.Tensor, scale: float) -> None:
+    """w[rows, cols] += scale * up[rows, rank] @ down[rank, cols] in place (include/ea_b200.h ea_lora_merge): w is bf16 or
+    float8_e4m3fn, up and down are both bf16 or both float32 (the compute dtype), all with a contiguous last dimension."""
+    for t, name in ((w, "w"), (up, "up"), (down, "down")):
+        if not t.is_cuda:
+            raise L.EaError(f"lora_merge: {name} must be a CUDA tensor (easyanimate_b200 has no CPU path)")
+    if w.dtype not in (bf16, torch.float8_e4m3fn):
+        raise L.EaError(f"lora_merge: w must be bfloat16 or float8_e4m3fn, got {w.dtype}")
+    if up.dtype != down.dtype or up.dtype not in (bf16, torch.float32):
+        raise L.EaError(f"lora_merge: up and down must both be bfloat16 or both float32, got {up.dtype} and {down.dtype}")
+    if w.dim() != 2 or up.dim() != 2 or down.dim() != 2 or up.shape[0] != w.shape[0] or down.shape[1] != w.shape[1] \
+            or up.shape[1] != down.shape[0]:
+        raise L.EaError(f"lora_merge: shapes w {tuple(w.shape)}, up {tuple(up.shape)}, down {tuple(down.shape)} do not chain")
+    if w.stride(1) != 1 or up.stride(1) != 1 or down.stride(1) != 1:
+        raise L.EaError("lora_merge: the last dimension of w, up and down must be contiguous")
+    if not w.device == up.device == down.device:
+        raise L.EaError("lora_merge: w, up and down must be on one device")
+    w_kind = L.LORA_W_E4M3 if w.dtype == torch.float8_e4m3fn else L.LORA_W_BF16
+    compute = L.LORA_C_F32 if up.dtype == torch.float32 else L.LORA_C_BF16
+    with torch.cuda.device(w.device):
+        L.check(L.ea_lora_merge(_p(w), _p(up), _p(down), w.shape[0], w.shape[1], up.shape[1], w.stride(0), up.stride(0),
+                                down.stride(0), scale, w_kind, compute, _stream()), "ea_lora_merge")
+
+
 def e4m3_segment_table(segments) -> tuple:
     """[(byte offset in the packed source, bf16 CUDA destination tensor)] -> the ctypes table expand_e4m3_segments takes.
     Build it once per (slot, staging block) pair: the destinations' addresses are baked in."""

@@ -209,6 +209,21 @@ int ea_h2d_block(void* dst, const void* src_host, int64_t bytes, void* wait_even
 int ea_expand_e4m3_segments(const void* src, const int64_t* src_offsets, void* const* dsts, const int64_t* counts,
                             int32_t n_segs, void* stream);
 
+/* LoRA merge (the reference's merge_lora / unmerge_lora, utils/lora_utils.py:424-430,486-492: the layer cast to the merge
+ * dtype c, W += multiplier * alpha * mm(up, down), cast back): W[rows, cols] += scale * up[rows, rank] · down[rank, cols] in
+ * place, in W's own storage.  up and down are in c (EA_LORA_C_*).  Per element, with rnd_c the rounding to c (none for fp32):
+ *   acc = fp32 FMA chain over k = 0 .. rank-1 in ascending order, starting from +0.0 (CUDA cores, no tensor cores)
+ *   d = rnd_c(acc);  d2 = rnd_c(fp32(scale * d));  w = rnd_c(fp32(W + d2));  W = storage(w)
+ * storage: bf16 round to nearest even, or float8_e4m3fn exactly as torch's .to(float8_e4m3fn) (nearest even, a magnitude
+ * rounding past 448 becomes NaN, no saturation).  Unmerge is the same call with -scale.  Strides in elements. */
+enum { EA_LORA_W_BF16 = 0, EA_LORA_W_E4M3 = 1 };
+enum { EA_LORA_C_BF16 = 0, EA_LORA_C_F32 = 1 };
+/* w [rows, cols] row stride ldw, updated in place; up [rows, rank] row stride ldu; down [rank, cols] row stride ldd.
+ * scale: multiplier * alpha / rank rounded to fp32, negative for unmerge.  w_kind: EA_LORA_W_BF16 | EA_LORA_W_E4M3.
+ * compute: EA_LORA_C_BF16 | EA_LORA_C_F32, the dtype of up / down and of the rounding points. */
+int ea_lora_merge(void* w, const void* up, const void* down, int64_t rows, int64_t cols, int64_t rank, int64_t ldw,
+                  int64_t ldu, int64_t ldd, float scale, int32_t w_kind, int32_t compute, void* stream);
+
 /* Joint text+video self-attention, non-causal, no mask, head_dim 64:  O = softmax(Q K^T * scale) V.
  * Replaces F.scaled_dot_product_attention + transpose/reshape/split at processor.py:287-303.
  * q,k,v: [B,H,S,64] bf16 contiguous.  Output is token-major and split at S_text:

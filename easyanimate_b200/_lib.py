@@ -160,7 +160,7 @@ ea_softmax_rows = _sig("ea_softmax_rows", [vp, vp, i64, i64, i64, i64, vp])
 ea_transpose2d = _sig("ea_transpose2d", [vp, vp, i64, i64, i64, i64, vp])
 ea_tile_blend = _sig("ea_tile_blend", [vp, i64, i64, i64, i64, vp, i64, i64, i64, i64, i64, i64, i32, vp])
 ea_copy2d = _sig("ea_copy2d", [vp, i64, i64, vp, i64, i64, i64, i64, i64, vp])
-ea_corner_blend = _sig("ea_corner_blend", [vp, vp, i64, i64, i64, i64, i64, vp])
+ea_corner_blend = _sig("ea_corner_blend", [vp, vp, i64, i64, i64, i64, i64, vp, vp, vp])
 
 
 def check(rc: int, what: str = "") -> None:

@@ -346,20 +346,20 @@ __global__ void copy2d_kernel(const bf16* __restrict__ src, int64_t s_plane, int
   dst[pl * d_plane + (int64_t)r * d_ld + c] = src[pl * s_plane + (int64_t)r * s_ld + c];
 }
 
-// lower-right corner re-blend (autoencoder_magvit.py:429-443): dst = w*src + (1-w)*dst, w = min(x/(W-1), y/(H-1))
+// lower-right corner re-blend (autoencoder_magvit.py:429-443): dst = w*src + (1-w)*dst, w = min(wx[c], wy[r]).
+// wx / wy are the reference's torch.linspace(0, 1, N) fp32 weights, built by the caller (no closed form here reproduces
+// torch's linspace for every N).  The reference combines fp32 tensors op by op, each product and sum rounded on its own:
+// the _rn intrinsics keep nvcc from contracting them into an FMA.  bf16 on store (the assignment into the bf16 video).
 __global__ void corner_blend_kernel(const bf16* __restrict__ src, bf16* __restrict__ dst, int64_t d_plane, int d_ld,
-                                    int planes, int Hc, int Wc) {
+                                    int planes, int Hc, int Wc, const float* __restrict__ wx, const float* __restrict__ wy) {
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= (int64_t)planes * Hc * Wc) return;
   const auto [pl, r, c] = planar_pos(idx, Hc, Wc);
-  // torch.linspace(0,1,N) in fp32: i * (1/(N-1)) evaluated symmetric; fp32 weights * bf16 -> fp32 math, bf16 on store
-  const float wx = Wc > 1 ? (float)c / (float)(Wc - 1) : 0.f;
-  const float wy = Hc > 1 ? (float)r / (float)(Hc - 1) : 0.f;
-  const float wgt = fminf(wx, wy);
+  const float wgt = fminf(__ldg(wx + c), __ldg(wy + r));
   const float s = __bfloat162float(src[(int64_t)pl * Hc * Wc + (int64_t)r * Wc + c]);
   bf16* dp = dst + pl * d_plane + (int64_t)r * d_ld + c;
   const float d = __bfloat162float(*dp);
-  *dp = __float2bfloat16_rn(wgt * s + (1.0f - wgt) * d);
+  *dp = __float2bfloat16_rn(__fadd_rn(__fmul_rn(wgt, s), __fmul_rn(__fsub_rn(1.0f, wgt), d)));
 }
 
 // decode_latents' tail (pipeline_easyanimate.py:729,738-740) on one decoded value: clamp(-1,1) -> /2 + 0.5 (two bf16 ops)
@@ -562,8 +562,8 @@ extern "C" int ea_copy2d(const void* src, int64_t s_plane, int64_t s_ld, void* d
 }
 
 extern "C" int ea_corner_blend(const void* src, void* dst, int64_t d_plane, int64_t d_ld, int64_t planes, int64_t Hc,
-                               int64_t Wc, void* stream) {
-  EA_REQUIRE(src && dst && planes > 0 && Hc > 0 && Wc > 0, "ea_corner_blend: bad arguments");
+                               int64_t Wc, const float* wx, const float* wy, void* stream) {
+  EA_REQUIRE(src && dst && wx && wy && planes > 0 && Hc > 0 && Wc > 0, "ea_corner_blend: bad arguments");
   return launch(corner_blend_kernel, grid_1d(planes * Hc * Wc, 256), 256, 0, stream, "corner_blend_kernel",
-                (const bf16*)src, (bf16*)dst, d_plane, (int)d_ld, (int)planes, (int)Hc, (int)Wc);
+                (const bf16*)src, (bf16*)dst, d_plane, (int)d_ld, (int)planes, (int)Hc, (int)Wc, wx, wy);
 }

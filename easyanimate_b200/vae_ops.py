@@ -219,11 +219,23 @@ def copy2d(src: torch.Tensor, dst: torch.Tensor, rows: int, cols: int, dst_r0: i
     L.check(L.ea_copy2d(_p(src), ps, ls, dptr, pd, ld, planes, rows, cols, _stream()), "ea_copy2d")
 
 
+_LINSPACE = {}  # (N, device) -> torch.linspace(0, 1, N) built on the host, as a float32 device vector
+
+
+def _linspace01(n: int, device: torch.device) -> torch.Tensor:
+    key = (n, device)
+    if key not in _LINSPACE:
+        _LINSPACE[key] = torch.linspace(0, 1, n).to(device)
+    return _LINSPACE[key]
+
+
 def corner_blend(src: torch.Tensor, dst: torch.Tensor) -> None:
-    """dst[..., -H:, -W:] = w*src + (1-w)*dst[..., -H:, -W:] (autoencoder_magvit.py:429-443)."""
+    """dst[..., -H:, -W:] = w*src + (1-w)*dst[..., -H:, -W:] (autoencoder_magvit.py:429-443), w = min(x_weights, y_weights)
+    with the reference's weights: torch.linspace(0, 1, N) evaluated on the CPU, which the kernel reads from two vectors."""
     planes = src.shape[0] * src.shape[1] * src.shape[2]
     Hc, Wc, Hd, Wd = src.shape[3], src.shape[4], dst.shape[3], dst.shape[4]
     assert src.is_contiguous()
     pd, ld = _planar(dst)
+    wx, wy = _linspace01(Wc, dst.device), _linspace01(Hc, dst.device)
     dptr = dst.data_ptr() + ((Hd - Hc) * ld + (Wd - Wc)) * 2
-    L.check(L.ea_corner_blend(_p(src), dptr, pd, ld, planes, Hc, Wc, _stream()), "ea_corner_blend")
+    L.check(L.ea_corner_blend(_p(src), dptr, pd, ld, planes, Hc, Wc, _p(wx), _p(wy), _stream()), "ea_corner_blend")

@@ -358,14 +358,17 @@ int ea_transpose2d(const void* in, void* out, int64_t R, int64_t C, int64_t ldi,
 
 /* tiled_decode blending (autoencoder_magvit.py:319-337,403-443) on planar [planes][H][W] images:
  * ea_tile_blend: b[r][c] = a[a_off_r+r][a_off_c+c]*(1-k/extent) + b[r][c]*(k/extent), k = r (axis 0) or c (axis 1)
- * ea_copy2d: strided crop/concat copy; ea_corner_blend: dst = w*src + (1-w)*dst, w = min(x/(W-1), y/(H-1)). */
+ * ea_copy2d: strided crop/concat copy;
+ * ea_corner_blend: dst[r][c] = w*src[r][c] + (1-w)*dst[r][c] with w = min(wx[c], wy[r]), every product and sum an fp32
+ *   op of its own, bf16 on store.  wx [Wc] / wy [Hc] are fp32 device vectors holding torch.linspace(0, 1, N) as torch
+ *   computes it on the CPU (autoencoder_magvit.py:430-431). */
 int ea_tile_blend(const void* a, int64_t a_plane, int64_t a_ld, int64_t a_off_r, int64_t a_off_c, void* b,
                   int64_t b_plane, int64_t b_ld, int64_t planes, int64_t rows, int64_t cols, int64_t extent,
                   int32_t axis, void* stream);
 int ea_copy2d(const void* src, int64_t s_plane, int64_t s_ld, void* dst, int64_t d_plane, int64_t d_ld, int64_t planes,
               int64_t rows, int64_t cols, void* stream);
 int ea_corner_blend(const void* src, void* dst, int64_t d_plane, int64_t d_ld, int64_t planes, int64_t Hc, int64_t Wc,
-                    void* stream);
+                    const float* wx, const float* wy, void* stream);
 
 #ifdef __cplusplus
 }

@@ -3,7 +3,8 @@ the argument conventions of the real wrappers (shapes, in-place outputs, row-per
 column order) and the rounding points documented in include/ea_b200.h, and for those of easyanimate_b200.vae_ops.
 TEST INFRASTRUCTURE: `use_stand_ins` installs them all, so that the CPU suite runs the product modules' HOST LOGIC (buffer
 plumbing, stream split, sequence-parallel sharding, decode dispatch) end to end without a GPU; they are never used by the
-product path."""
+product path.  tests/test_stand_ins_gpu.py holds each stand-in to its kernel (bit for bit where the op has no reduction or
+its inputs make every sum exact), and tests/test_stand_ins_cpu.py checks that every stand-in has such a case."""
 import math
 
 import torch
@@ -58,7 +59,7 @@ def layernorm_modulate(x, w, b, eps, *, shift=None, scale=None, rows_per_batch=0
     y = _r(y)
     if shift is not None:
         batch = torch.arange(x.shape[0]) // rows_per_batch
-        y = _r(_r(y * (1 + scale.float()[batch])) + shift.float()[batch])
+        y = _r(_r(y * _r(1 + scale.float()[batch])) + shift.float()[batch])  # 1 + scale is a bf16 tensor (norm.py:164)
     y = y.to(bf16)
     if out is not None:
         out.copy_(y)
@@ -176,12 +177,11 @@ def prepare_latents(z, w, b, cpad=64, in_scale=1.0):
 
 
 def groupnorm(x, gamma, beta, groups, eps, silu):
+    """Per-frame GroupNorm (common.py:301-305) with statistics from fp64 sums, as the kernel and torch's CUDA GroupNorm
+    (fp32 Welford) both get them to fp32 precision.  torch's CPU GroupNorm on this channels-last float32 input does not: on
+    data with a mean of 50 its output is off by up to 3e-3, close to a bf16 ulp."""
     T, H, W, C = x.shape
-    y = torch.nn.functional.group_norm(x.float().permute(0, 3, 1, 2), groups, gamma.float(), beta.float(), eps)  # per frame
-    y = _r(y)
-    if silu:
-        y = _r(torch.nn.functional.silu(y))
-    return y.permute(0, 2, 3, 1).contiguous().to(bf16)
+    return groupnorm_from_sums(x, groupnorm_sums(x, groups)[None], H * W * (C // groups), gamma, beta, groups, eps, silu)
 
 
 def groupnorm_sums(x, groups):
